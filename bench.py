@@ -1,21 +1,25 @@
 #!/usr/bin/env python
-"""bench.py -- VibeVoice generation hot path on B200: audio-seconds generated per wall-second.
+"""bench.py -- VibeVoice generation hot path on H100: audio-seconds generated per wall-second.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path (oracle port) on host cores
+    python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed as DIR/<name>.npy
 
 Workload (BASELINE.json configs[1], SURVEY 8d-2): VibeVoice-1.5B, 1 speaker, 64K context = 63,488-token synthetic prompt +
-2,047 generated speech frames (context ends at 65,535 = max_position_embeddings - 1; 273 s of audio per step), 30 diffusion
-steps, cfg 1.3, random-init weights, one prompt per GPU.  (`--prompt-len 61440 --frames 4095` gives SURVEY's variant.)
+128 generated speech frames per step (17 s of audio at a context of 63.5K tokens), 30 diffusion steps, cfg 1.3, random-init
+weights, one prompt per GPU.  A step is kept short so that --steps can repeat it many times; the per-frame work is the same as in
+a longer generation at that context.  (`--frames 2047` generates up to the 65,535-token limit in every step; `--prompt-len 61440
+--frames 4095` gives SURVEY's variant.)
 A "step" is one complete pass of the hot path over that prompt:
   value : K steps of the steady-state frame loop (LM decode pos+neg -> CFG diffusion sampler -> codec decode -> semantic
           encode -> connectors) with the prompt KV already resident in HBM; device-timed with CUDA events.
   e2e   : K calls of the public API `VibeVoiceForConditionalGenerationInference.generate()` with HOST input_ids: prompt
           prefill, per-frame token read-back and noise upload, and the waveform copied back to the host are all inside the
-          timed region.
+          timed region (the prefill of the 63.5K-token prompt is spread over the frames of one step).
 With N > 1 every rank runs the same workload on its own prompt (weak scaling; prompts shard by batch, SURVEY 8e); the only
-collective is the final NCCL gather of the waveforms to rank 0.  Frames stream ~13 GB of weights+KV each (>> 126 MB L2), so no
+collective is the final NCCL gather of the waveforms to rank 0.  Frames stream ~13 GB of weights+KV each (>> 50 MB L2), so no
 explicit L2 flush is needed between iterations ("inputs larger than L2").
+Every input (weights, prompt ids, per-frame noise) is drawn from fixed seeds, so two runs with the same arguments see the same inputs.
 """
 from __future__ import annotations
 
@@ -35,15 +39,13 @@ import numpy as np
 import torch
 
 AUDIO_S_PER_FRAME = 3200.0 / 24000.0
-# DRAM traffic of one frame / one LM step from an ncu pass (dram__bytes_read.sum + dram__bytes_write.sum over every kernel of the frame),
-# see profiles/ (filled in by the profiling run of this round; None = not captured for that model)
-TRAFFIC_NOTE = {
-    "1.5b": "10.96 GB DRAM (read + write) per frame for 12.98 GB algorithmic at ctx 61440: the four stream_kernel launches move 4.39 (LM stack: "
-            "4.40 algorithmic) + 5.02 (30-step sampler: 7.09 algorithmic, the rest of the head's re-reads hit the 126 MB L2) + 0.66 + 0.67 GB "
-            "(codec front / back), every other kernel 0.23 GB (ncu --set full + launch list of the final kernels, profiles/r02_prof_stream3_raw.csv, "
-            "profiles/r02_launches_15b_ctx61440_frame_final.txt)",
-    "1.5b:lm": "4.387 GB dram read + 0.012 GB written for 4.40 GB algorithmic (ncu --set full, profiles/r02_prof_stream3_raw.csv, launch 0)",
-}
+# HBM3 bandwidth of the H100 SXM data sheet; the roofline fraction uses MEASURED_PEAKS.json when it is present
+HBM_PEAK_GBS = 3350.0
+# speech frames generated per step of the 1.5B / 7B workloads (17 s of audio) unless --frames says otherwise
+FRAMES_PER_STEP = 128
+# largest total the --dump-outputs files may take (64 MB), .npy headers and the frame index included
+DUMP_CAP_BYTES = 64_000_000
+NPY_HEADER_BYTES = 128
 
 
 def parse():
@@ -63,11 +65,15 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-7b", action="store_true", help="skip the VibeVoice-7B sub-configs appended to the 1.5B line")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step of the steady-state loop computed (per-frame audio, latents, LM logits and "
+                         "tokens of every prompt) as DIR/<name>.npy in float32; a fixed, seeded sample of frames when the whole would "
+                         "exceed 64 MB.  The copies are enqueued inside that step.")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -155,7 +161,7 @@ def workload(args):
     maxpos = cfg.decoder_config.max_position_embeddings
     if args.model in ("1.5b", "7b"):
         L0 = args.prompt_len if args.prompt_len is not None else (63488 if args.model == "1.5b" else 30720)
-        F = args.frames if args.frames is not None else maxpos - 1 - L0
+        F = args.frames if args.frames is not None else min(FRAMES_PER_STEP, maxpos - 1 - L0)
     else:
         L0 = args.prompt_len or 64
         F = args.frames or 32
@@ -239,7 +245,7 @@ def config_dict(args, cfg, L0, F):
 
 # ------------------------------------------------------------------------------------------------------------------
 def run_extra_config(tag, preset, B, L0, F, args, rank, world, local, dev, peak):
-    """Steady-state loop of another BASELINE configuration (same method as `value`): 1 warm-up + 2 timed steps of F frames.
+    """Steady-state loop of another BASELINE configuration (same method as `value`): 1 warm-up + `--steps` timed steps of F frames.
     Every rank executes the same sequence of collectives whether or not its own part failed (a Python-level failure on one rank must
     not leave the others waiting in a barrier): failures are agreed on with a MIN all-reduce after each phase."""
     import torch.distributed as dist
@@ -274,7 +280,7 @@ def run_extra_config(tag, preset, B, L0, F, args, rank, world, local, dev, peak)
             for r in range(B):
                 model._prefill.run(eng, r, embw[ids[r].to(dev)])
         eng.sync()
-        noise_tab = torch.randn(F, B, 64, device=dev)
+        noise_tab = torch.randn(F, B, 64, device=dev, generator=torch.Generator(device=dev).manual_seed(400 + rank))
         ones = [1] * (2 * B)
 
         def step():
@@ -308,7 +314,7 @@ def run_extra_config(tag, preset, B, L0, F, args, rank, world, local, dev, peak)
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize(dev)
-    K = 2
+    K = args.steps
     ms = 0.0
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     try:
@@ -340,6 +346,37 @@ def run_extra_config(tag, preset, B, L0, F, args, rank, world, local, dev, peak)
     cleanup()
     del model, eng
     return out
+
+
+class DumpRecorder:
+    """Keeps what the frame loop hands a caller in one step -- per-frame audio [B, 3200], latent [B, 64], LM logits over the valid ids and
+    the constrained tokens -- for a fixed, seeded subset of frames (all of them when they fit DUMP_CAP_BYTES)."""
+
+    def __init__(self, eng, F, B, dev):
+        self.eng = eng
+        # float32 rows of the four outputs + the float64 frame index, per kept frame; 5 files' headers on top
+        per_frame = 4 * (eng.audio.numel() + eng.latent.numel() + eng.logits.numel() + eng.tokens.numel()) + 8
+        self.n_keep = max(1, min(F, (DUMP_CAP_BYTES - 5 * NPY_HEADER_BYTES) // per_frame))
+        keep = np.arange(F) if self.n_keep == F else np.sort(np.random.default_rng(0).choice(F, self.n_keep, replace=False))
+        self.slot = {int(f): i for i, f in enumerate(keep)}
+        self.frames = keep
+        z = lambda t: torch.zeros((self.n_keep,) + tuple(t.shape), dtype=torch.float32, device=dev)
+        self.bufs = {"audio": z(eng.audio), "latent": z(eng.latent), "logits": z(eng.logits), "tokens": z(eng.tokens)}
+
+    def frame(self, f):
+        i = self.slot.get(f)
+        if i is None:
+            return
+        with torch.cuda.stream(self.eng.stream):
+            for name, buf in self.bufs.items():
+                buf[i].copy_(getattr(self.eng, name))
+
+    def write(self, out_dir):
+        os.makedirs(out_dir, exist_ok=True)
+        self.eng.sync()
+        for name, buf in self.bufs.items():
+            np.save(os.path.join(out_dir, name + ".npy"), buf.cpu().numpy())
+        np.save(os.path.join(out_dir, "frames.npy"), self.frames.astype(np.float64))
 
 
 def run_b200(args):
@@ -380,10 +417,11 @@ def run_b200(args):
             model._prefill.run(eng, r, embw[ids[r].to(dev)])
     eng.sync()
     log("weights + prefill(%d tokens) done" % L0)
-    noise_tab = torch.randn(F, B, 64, device=dev)
+    noise_tab = torch.randn(F, B, 64, device=dev, generator=torch.Generator(device=dev).manual_seed(300 + rank))
     ones = [1] * (2 * B)
+    dump = DumpRecorder(eng, F, B, dev) if args.dump_outputs and rank == 0 else None
 
-    def value_step():
+    def value_step(record=None):
         eng.codec_state_reset()
         for r in range(B):
             eng.kv_set_len(r, L0); eng.kv_set_len(B + r, 0)
@@ -396,6 +434,8 @@ def run_b200(args):
             with torch.cuda.stream(eng.stream):
                 eng.noise.copy_(noise_tab[f])
             eng.frame_tail(args.cfg_scale)
+            if record is not None:
+                record.frame(f)
 
     for _ in range(W):
         value_step()
@@ -406,11 +446,14 @@ def run_b200(args):
     launches0 = eng.launch_count()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record(eng.stream)
-    for _ in range(K):
-        value_step()
+    for i in range(K):
+        value_step(dump if i == K - 1 else None)
     ev1.record(eng.stream)
     barrier()
     ms_value = ev0.elapsed_time(ev1)
+    if dump is not None:
+        dump.write(args.dump_outputs)
+        log("outputs of the last timed step written to %s" % args.dump_outputs)
     log("value timed: %.1f ms for %d steps" % (ms_value, K))
     launches = eng.launch_count() - launches0
     clk = clocks.stop()
@@ -430,10 +473,10 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     achieved = abytes / (ms_frame * 1e-3) / 1e9
     roofline = {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                "traffic": None, "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+                "traffic": None, "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3350 GB/s",
                 "unit_of_work": "one speech frame = lm_decode graph + frame_tail graph",
                 "algorithmic_bytes_per_frame": int(abytes), "ms_per_frame": round(ms_frame, 4)}
 
@@ -471,14 +514,12 @@ def run_b200(args):
         return out
     segs = segment_rooflines()
     roofline["segments"] = segs
-    roofline["traffic"] = TRAFFIC_NOTE.get(args.model)
     lm_seg = segs["lm_decode"]
     roofline["dominant_kernel"] = {
-        "kernel": "stream_kernel (vv_stream.cuh): the whole %d-layer decoder stack of one step as ONE persistent launch -- tcgen05.mma + TMEM, "
-                  "weight tiles and K/V pages by TMA through one ring" % cfg.decoder_config.num_hidden_layers,
+        "kernel": "stream_kernel (vv_stream.cuh): the whole %d-layer decoder stack of one step as ONE persistent launch -- wgmma with register "
+                  "accumulators, weight tiles and K/V pages by TMA through one ring" % cfg.decoder_config.num_hidden_layers,
         "bound": "hbm", "achieved": lm_seg["achieved_GBps"], "peak": peak, "unit": "GB/s", "frac": lm_seg["frac"],
         "algorithmic_bytes_per_launch": lm_seg["algorithmic_bytes"], "us_per_launch": lm_seg["us"],
-        "traffic": TRAFFIC_NOTE.get(args.model + ":lm"),
         "note": "vv_lm_decode timed alone (copy-in, the stream launch, final norm, 4-row lm_head); weights + KV of one step >> L2"}
     head_step_us = segs["diffusion_sample"]["us"] / args.diffusion_steps
     log("segment rooflines done")
@@ -558,6 +599,8 @@ def run_b200(args):
                 "diffusion_head_step_floor_us": round(wb["head_step"] / peak / 1e3, 2),
                 "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches), "clocks": clk, "configs": extra_configs,
                 "weight_bytes": wb, "setup_s": round(time.time() - t_setup, 1)}
+        if dump is not None:
+            line["dump_outputs"] = {"dir": args.dump_outputs, "frames": dump.n_keep, "of_frames": F}
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()

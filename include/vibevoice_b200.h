@@ -1,11 +1,11 @@
 /*
- * vibevoice_b200.h -- C ABI of libvibevoice_b200.so (hand-written sm_100a kernels + native runtime).
+ * vibevoice_b200.h -- C ABI of libvibevoice_b200.so (hand-written sm_90a kernels + native runtime).
  *
  * The reference (vibevoice-community/VibeVoice) is 100% Python/PyTorch and has no FFI layer; its
  * boundary for this path is the Python surface of
  *   vibevoice/modular/modeling_vibevoice_inference.py:68   VibeVoiceForConditionalGenerationInference
  * This header is the boundary a drop-in replacement binds instead (via ctypes, see INTEGRATION.md):
- * every entry point below names the reference code it replaces (file:line under /root/reference).
+ * every entry point below names the reference code it replaces (file:line in vibevoice-community/VibeVoice).
  *
  * Conventions
  *   - plain C: opaque handle, raw pointers, sizes; no torch / C++ types.
@@ -163,14 +163,13 @@ int vv_debug_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const floa
                   int prologue, const float* pro_w, float eps, int epilogue, void* stream);
 
 int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_out);
-/* one linear through the persistent weight-stream kernel (tcgen05 + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).
+/* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).
  * prologue: 0 none, 1 RMSNorm(pro_w, eps), 3 SwiGLU pairs (x is [M][2K]), 4 GELU, 6 SiLU; alpha_kind: 0 one, 2 gamma[n]. Synchronises. */
 int vv_debug_stream_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, float* y, int M, int N, int K, int prologue,
                          const float* pro_w, float eps, int alpha_kind, const float* alpha, int accumulate, void* stream);
 int vv_stream_trace_read2(vv_ctx* ctx, long long* out /*[max_ops][sm_count][2]*/, int max_ops);  /* every CTA's barrier arrival / release (globaltimer ns); returns sm_count */
 int vv_stream_trace_read(vv_ctx* ctx, long long* out /*[max_ops][12]*/, int* out_meta /*[max_ops][4]*/, int max_ops, const char* program_prefix);
                                                    /* VV_STREAM_TRACE=<cta>: per-stage clock stamps of one CTA of the last traced launch */
-int vv_debug_mma_rate(vv_ctx* ctx, int n_mma, int nB, int mode, int n_accumulators, int ctas, long long* cycles_out);   /* tcgen05.mma 128 x nB x 16 micro-benchmark */
 int vv_stream_diag(vv_ctx* ctx, unsigned* out6);   /* watchdog record of a trapped stream kernel: code, cta, thread, stage, iteration, extra */
 
 #ifdef __cplusplus

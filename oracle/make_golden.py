@@ -1,11 +1,11 @@
 """TEST INFRASTRUCTURE -- generates `tests/golden/*.pt` by running the UNMODIFIED reference modules
-(imported from /root/reference through `oracle/ref_shim.py`) on seeded synthetic checkpoints.
+(imported from the reference checkout named by VV_REFERENCE_ROOT through `oracle/ref_shim.py`) on seeded synthetic checkpoints.
 
-    python -m oracle.make_golden [name ...]   # rewrites tests/golden/ (all fixtures, or the named ones)
+    VV_REFERENCE_ROOT=<reference checkout> python -m oracle.make_golden [name ...]   # rewrites tests/golden/ (all, or the named ones)
 
 The reference has no golden vectors of its own (SURVEY section 4); these fixtures are what pins the oracle
-(`oracle/vv_oracle.py`) and, through it, the CUDA path.  Only runs in the build container (the GPU box
-has no /root/reference); the fixtures it writes are committed.
+(`oracle/vv_oracle.py`) and, through it, the CUDA path.  Only runs where the reference checkout exists;
+the fixtures it writes are committed, so the tests never need the reference.
 """
 from __future__ import annotations
 
@@ -232,6 +232,21 @@ def _scripted(tok, s):
     return [m[c] for c in s]
 
 
+def _chunks_as_views(items, audio):
+    """Streamed chunks [1, 3200] (None = stop signal) as views of the row's waveform when they concatenate to it exactly."""
+    chunks = [c for c in items if c is not None]
+    if audio is None or not chunks or not torch.equal(torch.cat(chunks, -1), audio):
+        return items
+    out, t = [], 0
+    for c in items:
+        if c is None:
+            out.append(None)
+        else:
+            out.append(audio.narrow(-1, t, c.shape[-1]))
+            t += c.shape[-1]
+    return out
+
+
 def gen_loop(ns, preset="tiny"):
     """The reference's own `generate()` (modeling_vibevoice_inference.py:326-695), loop body unmodified, on the synthetic tiny
     checkpoint; transformers-4.51.3 GenerationMixin glue restated by `ref_shim.install_generate_compat()`.  Three cases:
@@ -286,10 +301,12 @@ def gen_loop(ns, preset="tiny"):
                     it = q.get()
                     items.append(None if it is None else it.clone())
                 streamed.append(items)
+        audio = [None if a is None else a.clone() for a in out.speech_outputs]
+        if streamed is not None:                     # chunks that make up a row's waveform are stored once, as views of it
+            streamed = [_chunks_as_views(items, audio[i]) for i, items in enumerate(streamed)]
         return dict(streamed=streamed, stop_after_calls=stop_after_calls,
                     ids=ids, mask=mask, scripts=scripts, max_new_tokens=max_new_tokens, seed=seed, max_length_times=max_length_times, refresh_negative=refresh_negative, do_sample=do_sample,
-                    sequences=out.sequences.clone(), reach_max=out.reach_max_step_sample.clone(),
-                    audio=[None if a is None else a.clone() for a in out.speech_outputs])
+                    sequences=out.sequences.clone(), reach_max=out.reach_max_step_sample.clone(), audio=audio)
 
     g = torch.Generator().manual_seed(3)
     L0 = 12
@@ -421,7 +438,42 @@ def gen_streaming(ns, preset="tiny"):
     return out
 
 
-GENERATORS = dict(streaming=gen_streaming, loop=gen_loop, voice_prompt=gen_voice_prompt, scheduler=gen_scheduler, head=gen_head, codec=gen_codec, connector=gen_connector, lm=gen_lm)
+def gen_processor(ns):
+    """The reference's VibeVoiceProcessor (vibevoice/processor/vibevoice_processor.py) on the inputs of tests/test_processor.py: a batch
+    of two scripts with voice prompts, and one script without."""
+    import importlib.util
+    import numpy as np
+    spec_t = importlib.util.spec_from_file_location("vv_test_processor_inputs", os.path.join(ROOT, "tests", "test_processor.py"))
+    tp = importlib.util.module_from_spec(spec_t); spec_t.loader.exec_module(tp)
+    SCRIPT, StubTokenizer, _voices = tp.SCRIPT, tp.StubTokenizer, tp._voices
+    base = os.path.join(ref_shim.REFERENCE_ROOT, "vibevoice", "processor")
+    # this repository's drop-in alias package shadows the reference's on sys.path: load the reference files explicitly
+    spec0 = importlib.util.spec_from_file_location("refproc.vibevoice_tokenizer_processor", os.path.join(base, "vibevoice_tokenizer_processor.py"))
+    m0 = importlib.util.module_from_spec(spec0); sys.modules[spec0.name] = m0; spec0.loader.exec_module(m0)
+    src = open(os.path.join(base, "vibevoice_processor.py")).read().replace("from .vibevoice_tokenizer_processor", "from refproc.vibevoice_tokenizer_processor")
+    rp = types.ModuleType("refproc.vibevoice_processor"); rp.__file__ = os.path.join(base, "vibevoice_processor.py")
+    sys.modules.setdefault("refproc", types.ModuleType("refproc"))
+    exec(compile(src, rp.__file__, "exec"), rp.__dict__)
+    ref = rp.VibeVoiceProcessor(tokenizer=StubTokenizer(), audio_processor=None)
+    keep = ("input_ids", "attention_mask", "speech_input_mask", "speech_masks", "speech_tensors", "parsed_scripts")
+    a = ref(text=[SCRIPT, "Speaker 0: Hi."], voice_samples=[_voices(), [_voices()[0]]], padding=True, return_tensors="pt")
+    a2 = ref(text=SCRIPT, padding=True, return_tensors="pt")
+    conv = lambda v: torch.as_tensor(np.asarray(v)) if isinstance(v, np.ndarray) else v
+    return {"batch": {k: conv(a[k]) for k in keep}, "single": {"input_ids": conv(a2["input_ids"]), "speech_tensors": a2["speech_tensors"]}}
+
+
+def gen_configs(ns):
+    """The shipped model configuration JSON of VibeVoice-1.5B (vibevoice/configs/qwen2.5_1.5b_64k.json), as data."""
+    import json
+    with open(os.path.join(ref_shim.REFERENCE_ROOT, "vibevoice", "configs", "qwen2.5_1.5b_64k.json")) as f:
+        return {"qwen2.5_1.5b_64k": json.load(f)}
+
+
+# fixtures written as two files (every file stays below 1 MB): these cases of `name` go to `<name>2.pt`, the rest to `<name>.pt`
+SPLIT = {"loop": ("voice", "streamed", "stopped", "sde")}
+
+GENERATORS = dict(streaming=gen_streaming, loop=gen_loop, voice_prompt=gen_voice_prompt, scheduler=gen_scheduler, head=gen_head, codec=gen_codec, connector=gen_connector, lm=gen_lm,
+                  processor=gen_processor, configs=gen_configs)
 
 
 def main():
@@ -433,9 +485,13 @@ def main():
             continue
         torch.manual_seed(0)
         data = fn(ns)
-        path = os.path.join(GOLDEN_DIR, f"{name}.pt")
-        torch.save(data, path)
-        print("wrote", path, os.path.getsize(path), "bytes")
+        parts = {name: data}
+        if name in SPLIT:
+            parts = {name: {k: v for k, v in data.items() if k not in SPLIT[name]}, name + "2": {k: data[k] for k in SPLIT[name]}}
+        for fname, part in parts.items():
+            path = os.path.join(GOLDEN_DIR, f"{fname}.pt")
+            torch.save(part, path)
+            print("wrote", path, os.path.getsize(path), "bytes")
 
 
 if __name__ == "__main__":

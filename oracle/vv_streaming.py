@@ -1,7 +1,7 @@
 """CPU ORACLE (TEST INFRASTRUCTURE) for the streaming-0.5B variant -- SURVEY 8f-1, the first "next" row.
 
 Restates `VibeVoiceStreamingForConditionalGenerationInference.generate`
-(/root/reference/vibevoice/modular/modeling_vibevoice_streaming_inference.py:412-725) on a flat state dict with the reference's key
+(reference vibevoice/modular/modeling_vibevoice_streaming_inference.py:412-725) on a flat state dict with the reference's key
 names, reusing the arithmetic of `vv_oracle` (Qwen2 stack, diffusion head + DPM-Solver++, streaming acoustic decoder, connector).
 Pinned against the reference's own generate() on a synthetic checkpoint: `tests/golden/streaming.pt` (`oracle/make_golden.py::
 gen_streaming`), held by `tests/test_oracle_golden.py::test_streaming_generate_matches_the_reference`.

@@ -2,7 +2,7 @@
 paths (`vibevoice.modular.modeling_vibevoice_inference`, `vibevoice.processor.vibevoice_processor`), on a synthetic checkpoint directory:
 sharded safetensors with the reference's key names + `config.json` in the shipped format + `preprocessor_config.json` + tokenizer files,
 two voice wavs on disk (one at 16 kHz: the shipped `en-Alice_woman.wav` is), a script file.  The calls and keyword arguments are the
-demo's, unmodified; only the model path differs.  (`/root/reference` does not exist on the GPU box, so the flow is restated here.)"""
+demo's, unmodified; only the model path differs.  (The tests do not depend on a reference checkout, so the flow is restated here.)"""
 import json
 import os
 

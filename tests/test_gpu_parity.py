@@ -20,7 +20,8 @@ from vibevoice_b200.configuration import preset_config
 from vibevoice_b200.synth import SynthTokenizer, synth_state_dict
 
 SEED = 1234
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+# per-test error figures, appended as JSON lines (VV_REPORT_DIR, default reports/ in the repository)
+OUT = os.environ.get("VV_REPORT_DIR") or os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "reports")
 
 
 def rel_l2(a: torch.Tensor, b: torch.Tensor) -> float:
@@ -677,19 +678,19 @@ def test_voice_prompt_and_torch_prefill_vs_oracle():
     model.engine.close()
 
 
-def test_tcgen05_gemm_forced_everywhere():
-    """gemm_tc5_kernel (tcgen05.mma + TMEM accumulator) is selected automatically only for wide GEMMs; force it for EVERY
-    M > 8 GEMM (VV_TC5=2) and re-check the GEMM-vs-torch cases and a closed codec loop through the tensor-core path."""
+def test_wgmma_gemm_forced_everywhere():
+    """gemm_wgmma_kernel (warpgroup wgmma.mma_async, register accumulators) is selected automatically only for wide GEMMs; force it for
+    EVERY M > 8 GEMM (VV_WGMMA=2) and re-check the GEMM-vs-torch cases and a closed codec loop through the tensor-core path."""
     import ctypes as C
-    old = os.environ.get("VV_TC5")
-    os.environ["VV_TC5"] = "2"
+    old = os.environ.get("VV_WGMMA")
+    os.environ["VV_WGMMA"] = "2"
     try:
         m, cfg, tok, sd = make_model("tiny", 1)
     finally:
         if old is None:
-            os.environ.pop("VV_TC5", None)
+            os.environ.pop("VV_WGMMA", None)
         else:
-            os.environ["VV_TC5"] = old
+            os.environ["VV_WGMMA"] = old
     eng = m.engine
     P = lambda t: C.c_void_p(t.data_ptr())
     for (M, N, K) in [(40, 2048, 512), (200, 1024, 256), (70, 96, 40), (60, 21504, 1536), (130, 200, 72)]:
@@ -707,7 +708,7 @@ def test_tcgen05_gemm_forced_everywhere():
             ref = x @ W.float().T + bias
             ref = torch.nn.functional.gelu(ref) if epi == NV.EPI_GELU else (ref + 0.25 if epi == NV.EPI_RESID else ref)
             e = rel_l2(y, ref)
-            report("tc5_gemm", M=M, N=N, K=K, epi=epi, rel_l2=e)
+            report("wgmma_gemm", M=M, N=N, K=K, epi=epi, rel_l2=e)
             assert e < 2e-5, (M, N, K, epi, e)
     from oracle import vv_oracle as O
     eng.codec_state_reset()

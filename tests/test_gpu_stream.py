@@ -1,4 +1,4 @@
-"""`-m gpu`: the persistent weight-stream kernel (tcgen05.mma + TMEM accumulators, weight tiles by TMA through a ring that runs across
+"""`-m gpu`: the persistent weight-stream kernel (wgmma with register accumulators, weight tiles by TMA through a ring that runs across
 grid barriers; csrc/vv_stream.cuh) against a plain PyTorch fp32 reference of the same op.  Activations are split into bf16 hi + lo
 inside the kernel, weights are bf16 on both sides -> agreement to ~1e-5 (summation order, 2^-17 relative activation rounding)."""
 import ctypes as C

@@ -64,7 +64,7 @@ def test_scheduler_rejects_variants_off_the_path():
     assert s2.config.solver_order == 2
 
 
-def test_configs_match_the_shipped_jsons():
+def test_configs_match_the_shipped_jsons(golden, tmp_path):
     from vibevoice_b200.configuration import VibeVoiceConfig, preset_config
     from vibevoice_b200.synth import param_specs
     import math
@@ -73,11 +73,12 @@ def test_configs_match_the_shipped_jsons():
         assert sum(math.prod(s) for _, s, _ in param_specs(cfg)) == n_params
     c = preset_config("1.5b")
     assert c.acoustic_tokenizer_config.decoder_depth_list == [8, 3, 3, 3, 3, 3, 3]
-    ref = "/root/reference/vibevoice/configs/qwen2.5_1.5b_64k.json"
-    if os.path.exists(ref):
-        r = VibeVoiceConfig.from_pretrained(ref)
-        assert r.decoder_config.hidden_size == 1536 and r.decoder_config.num_key_value_heads == 2
-        assert r.diffusion_head_config.head_layers == 4 and r.semantic_vae_dim == 128
+    import json
+    ref = tmp_path / "config.json"          # the shipped 1.5B JSON, stored as a fixture (tests/golden/configs.pt)
+    ref.write_text(json.dumps(golden("configs")["qwen2.5_1.5b_64k"]))
+    r = VibeVoiceConfig.from_pretrained(str(ref))
+    assert r.decoder_config.hidden_size == 1536 and r.decoder_config.num_key_value_heads == 2
+    assert r.diffusion_head_config.head_layers == 4 and r.semantic_vae_dim == 128
 
 
 def test_shard_prompts():
@@ -224,7 +225,7 @@ def test_product_generate_host_logic_against_reference_generate_fixture(golden, 
     from vibevoice_b200.configuration import preset_config
     from vibevoice_b200.modeling import ForcedTokenScript
     from vibevoice_b200.synth import SynthTokenizer, synth_state_dict
-    g = golden("loop")
+    g = {**golden("loop"), **golden("loop2")}          # the loop fixture is stored in two files
     c = g[case]
     cfg = preset_config(g["preset"])
     tok = SynthTokenizer(cfg.decoder_config.vocab_size)
@@ -266,7 +267,7 @@ def test_product_streaming_and_stop_hooks_against_reference_generate_fixture(gol
     from vibevoice_b200.modeling import ForcedTokenScript
     from vibevoice_b200.streamer import AudioStreamer
     from vibevoice_b200.synth import SynthTokenizer, synth_state_dict
-    g = golden("loop")
+    g = {**golden("loop"), **golden("loop2")}          # the loop fixture is stored in two files
     c = g[case]
     cfg = preset_config(g["preset"])
     tok = SynthTokenizer(cfg.decoder_config.vocab_size)

@@ -122,7 +122,7 @@ def test_generate_loop_matches_the_reference_generate(golden, case):
     (loop body unmodified; transformers-4.51.3 glue restated in `oracle/ref_shim.py::install_generate_compat`).
     Token sequences and reach_max flags: exact.  Waveforms: fp32 on both sides, 1e-5."""
     from vibevoice_b200.synth import SynthTokenizer
-    g = golden("loop")
+    g = {**golden("loop"), **golden("loop2")}          # the loop fixture is stored in two files
     c = g[case]
     cfg = preset_config(g["preset"])
     tok = SynthTokenizer(cfg.decoder_config.vocab_size)
@@ -157,7 +157,7 @@ def test_logical_negative_bookkeeping_is_the_reference_on_well_formed_sequences(
     is bit-identical to the reference-faithful bookkeeping on well-formed sequences, and differs on the one ill-formed pattern
     where the reference's two guards disagree (:603 vs :613) -- a stated deviation of the product path (DESIGN section 4)."""
     from vibevoice_b200.synth import SynthTokenizer
-    g = golden("loop")
+    g = {**golden("loop"), **golden("loop2")}          # the loop fixture is stored in two files
     cfg = preset_config(g["preset"])
     tok = SynthTokenizer(cfg.decoder_config.vocab_size)
     sd = synth_state_dict(cfg, SEED, torch.float32)

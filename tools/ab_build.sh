@@ -3,6 +3,6 @@
 set -e
 cd "$(dirname "$0")/.."; mkdir -p ab
 name=$1; shift
-/usr/local/cuda/bin/nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC -shared "$@" \
+/usr/local/cuda/bin/nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC -shared "$@" \
   vibevoice_b200/csrc/vv_runtime.cu -o ab/lib_$name.so
 echo ab/lib_$name.so

@@ -1,5 +1,6 @@
 """Micro-benchmark of the weight-streaming GEMV through the C ABI (vv_debug_gemv): achieved HBM GB/s per shape,
-timed with CUDA events over back-to-back launches that rotate through enough weight copies to defeat the 126 MB L2."""
+timed with CUDA events over back-to-back launches that rotate through ~400 MB of weight copies,
+far more than the H100's 50 MB L2."""
 import ctypes as C
 import json
 import os
@@ -45,5 +46,6 @@ for M, N, K, pro, epi in shapes:
     out.append(rec)
     print(rec, flush=True)
     del W
-json.dump(out, open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out",
+os.makedirs(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "reports"), exist_ok=True)
+json.dump(out, open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "reports",
                                  "gemv_bench_%s.json" % ("notma" if os.environ.get("VV_NO_TMA") == "1" else "tma")), "w"))

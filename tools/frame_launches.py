@@ -1,6 +1,6 @@
 """One frame out of an `ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --csv` launch list of
 `tools/profile_frame.py` (all kernels captured, no -k filter: ncu's filter matches unqualified names only):
-    python tools/frame_launches.py gpurun_out/launches.csv profiles/out_prefix
+    python tools/frame_launches.py launches.csv out/prefix
 keeps the launches from one LM-stack `stream_kernel` launch to the next (= one speech frame), drops the one-time weight-packing
 kernels of the first frame, writes <prefix>.csv (the kept rows) and <prefix>.txt (per-kernel counts, time shares, DRAM bytes)."""
 import collections

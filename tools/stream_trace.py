@@ -86,7 +86,7 @@ for key, v in rows.items():
 print("inside 'stats' (norm stages): loads issued %.2f us, first row pair reduced %.2f us after the barrier" % (
     np.median([us(out[i][10] - out[i][1]) for i in range(n) if meta[i][3] in (1, 2) and out[i][10]]),
     np.median([us(out[i][11] - out[i][1]) for i in range(n) if meta[i][3] in (1, 2) and out[i][11]])))
-G = 148
+G = torch.cuda.get_device_properties(0).multi_processor_count     # one stream-kernel CTA per SM
 t2 = np.zeros((MAXO, G, 2), dtype=np.int64)
 G = eng.lib.vv_stream_trace_read2(eng.h, t2.ctypes.data_as(C.c_void_p), MAXO)
 if G:

@@ -1,4 +1,4 @@
-"""`vibevoice/modular/modeling_vibevoice_inference.py` import path -> B200 implementation."""
+"""`vibevoice/modular/modeling_vibevoice_inference.py` import path -> H100 implementation."""
 from vibevoice_b200.modeling import ForcedTokenScript, VibeVoiceForConditionalGenerationInference, VibeVoiceGenerationOutput  # noqa: F401
 
 __all__ = ["VibeVoiceForConditionalGenerationInference"]

@@ -79,7 +79,6 @@ SYMBOLS = {
     "vv_debug_gemv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _F, _I, _P]),
     "vv_debug_stream_gemv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _F, _I, _P, _I, _P]),
     "vv_stream_diag": (_I, [_P, _P]),
-    "vv_debug_mma_rate": (_I, [_P, _I, _I, _I, _I, _I, _P]),
     "vv_stream_trace_read": (_I, [_P, _P, _P, _I, C.c_char_p]),
     "vv_stream_trace_read2": (_I, [_P, _P, _I]),
 }

@@ -1,4 +1,4 @@
-"""Builds libvibevoice_b200.so for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+"""Builds libvibevoice_b200.so for sm_90a (H100) in-tree (nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "libvibevoice_b200.so")
 SOURCES = ["vv_runtime.cu"]
-FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",
          "-shared", "--use_fast_math=false", "-Xptxas", "-v"]
 
 

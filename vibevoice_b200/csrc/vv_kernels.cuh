@@ -1,4 +1,4 @@
-// vv_kernels.cuh -- hand-written sm_100a kernels of the VibeVoice generation hot path.
+// vv_kernels.cuh -- hand-written sm_90a kernels of the VibeVoice generation hot path.
 //
 // Everything in the per-frame loop runs at M <= 2B rows against bf16 weight matrices, i.e. it is
 // HBM-bandwidth bound (SURVEY 8d): the kernels below stream each weight byte exactly once with
@@ -6,7 +6,7 @@
 // fp32 and fuse the surrounding norm / modulation / activation / residual work into the GEMV
 // prologue and epilogue so no activation round-trips through HBM more than once.
 //
-// Reference anchors (under /root/reference/vibevoice/modular unless noted):
+// Reference anchors (under vibevoice/modular of the reference project unless noted):
 //   gemv prologues RMSNORM/ADALN      modular_vibevoice_diffusion_head.py:31-45, 158-161, 184-188;
 //                                     transformers Qwen2RMSNorm (modeling_qwen2.py:249-266)
 //   gemv epilogues SWIGLU/GATED_RESID modular_vibevoice_diffusion_head.py:116-123, 158-161
@@ -332,7 +332,7 @@ __global__ void __launch_bounds__(256) gemv_kernel(GemvP p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// mbarrier / bulk-copy primitives (shared by the tcgen05 GEMM below and the weight-stream kernel in vv_stream.cuh)
+// mbarrier / bulk-copy primitives (shared by the weight-stream kernel in vv_stream.cuh)
 // ---------------------------------------------------------------------------------------------
 VV_DEVINL unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 VV_DEVINL void mbar_init(unsigned long long* bar, int count) {
@@ -364,7 +364,7 @@ VV_DEVINL void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); 
 // 2^-16 relative), W is bf16, so two bf16 MMAs per tile reproduce the fp32-activation result of
 // the GEMV path to ~1e-5 while running on the tensor pipe.  CTA tile 32 x 64 x 64, 4 warps, W
 // streamed with a 3-stage cp.async ring, A register-prefetched one k-step ahead.
-// (mma.sync m16n8k16; the tcgen05/TMEM version of this kernel is the planned replacement.)
+// (mma.sync m16n8k16.)
 // ---------------------------------------------------------------------------------------------
 VV_DEVINL void cp_async16(void* smem, const void* gmem, int src_bytes) {
   unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
@@ -522,8 +522,7 @@ __global__ void __launch_bounds__(128) gemm_mma_kernel(GemvP p) {
 // ---------------------------------------------------------------------------------------------
 // Deep-ring variant of gemm_mma_kernel for the codec GEMMs with M > 8 (FFNs, transposed convs); prologue none or RMSNorm.
 // Why: these GEMMs are tiny (K = 32..2048, <= 112 CTAs) and each CTA used to pay one L2/DRAM round trip PER k-step
-// (A register-prefetched one step ahead, W two steps ahead: ~3300 cycles per 64-wide k-step in ncu, 13-30 us per launch for a few
-// MFLOP).  Here BOTH operands arrive by cp.async into a 6-stage ring -- fp32 A tile [32 x 64] and bf16 W tile [64 x 64] per stage --
+// (A register-prefetched one step ahead, W two steps ahead).  Here BOTH operands arrive by cp.async into a 6-stage ring -- fp32 A tile [32 x 64] and bf16 W tile [64 x 64] per stage --
 // so up to five k-steps (usually the whole K of a split) are in flight from the first instruction and a CTA pays ~one round trip in
 // total.  The fp32 A tile is converted to the bf16 hi/lo mma fragments straight from shared memory (LDS.64 per fragment register,
 // row stride 72 floats = conflict-free), which also removes the second __syncthreads and the Ah/Al staging of the old kernel.
@@ -535,8 +534,7 @@ constexpr int MR_SMEM = MR_ST * MR_STAGE;
 constexpr int MR_MAXK_NORM = 512;                  // PRO_RMSNORM: the norm weight row is staged in shared memory behind the ring (2 CTAs/SM must still fit)
 constexpr int MR_SMEM_NORM = MR_SMEM + MR_MAXK_NORM * 4;
 // RMS / EPI >= 0: prologue and epilogue kind as compile-time facts (the codec tail launches this kernel 68 times per frame and every
-// launch runs its path once from a cold instruction cache: ncu shows 1.2-2.6 `no_instruction` stalls per issued instruction for the
-// run-time-switched version); -1 = decided at run time.
+// launch runs its path once from a cold instruction cache); -1 = decided at run time.
 template <int RMS, int EPI>
 __global__ void __launch_bounds__(128) gemm_mma_ring_kernel(GemvP p) {
   extern __shared__ __align__(16) unsigned char mr_smem[];
@@ -665,31 +663,48 @@ __global__ void __launch_bounds__(128) gemm_mma_ring_kernel(GemvP p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM GEMM (5th-gen tensor cores) for the M > 8 GEMMs: D^T[128 x 64] += W[128 x K] * A[64 x K]^T ("swap-AB":
-// the 128-row MMA M dimension is filled with weight rows, the MMA N dimension with up to 64 activation rows).
-//   * operands in shared memory, K-major, 128-byte swizzle (canonical UMMA layout ((8,n),2):((8,SBO),1), SBO = 1024 B);
-//     W tiles and the activation planes arrive by cp.async into swizzled positions (three stages, requested two k-blocks ahead);
-//     activations are pre-split fp32 -> bf16 hi + bf16 lo (split_bf16_kernel) and both halves are multiplied into the SAME
-//     accumulator (two MMAs), so the result keeps ~fp32-activation accuracy;
-//   * accumulator in TMEM (64 fp32 columns x 128 lanes), one elected thread issues tcgen05.mma, completion is tracked with
-//     tcgen05.commit on an mbarrier, two shared-memory stages are in flight;
-//   * epilogue: tcgen05.ld 32x32b (warp w owns TMEM lanes 32w..32w+31 = weight rows), fused bias / activation / residual.
-// SASS: UTCHMMA (tcgen05.mma), LDTM (tcgen05.ld), UTCBAR (commit).
+// Warpgroup GEMM (Hopper wgmma) for the wide M > 8 GEMMs: D^T[128 x 64] += W[128 x K] * A[64 x K]^T ("swap-AB": the weight rows fill
+// the MMA M dimension as two m64 halves, the MMA N dimension holds up to 64 activation rows).
+//   * operands in shared memory, K-major, 128-byte swizzle (8-row atoms of 8 x 128 B, stride byte offset 1024 B); W tiles and the
+//     activation planes arrive by cp.async into swizzled positions (three stages, requested two k-blocks ahead); activations are
+//     pre-split fp32 -> bf16 hi + bf16 lo (split_bf16_kernel) and both halves are multiplied into the SAME accumulator (two MMAs),
+//     so the result keeps ~fp32-activation accuracy;
+//   * the CTA is one warpgroup: wgmma.mma_async m64n64k16 from shared memory, fp32 accumulators in registers (64 per thread);
+//   * epilogue straight from the accumulator fragments, fused bias / activation / residual.
 // ---------------------------------------------------------------------------------------------
-constexpr int T5_BM = 128, T5_BN = 64, T5_BK = 64;
-constexpr int T5_STAGE = T5_BM * 128 + 2 * T5_BN * 128;          // W 16 KB + A_hi 8 KB + A_lo 8 KB
-constexpr int T5_NST = 3;                                       // shared-memory stages (weights are requested two k-blocks ahead)
-constexpr int T5_SMEM = T5_NST * T5_STAGE + 1024;               // + slack for 1024 B alignment
+constexpr int WG_BM = 128, WG_BN = 64, WG_BK = 64;
+constexpr int WG_STAGE = WG_BM * 128 + 2 * WG_BN * 128;          // W 16 KB + A_hi 8 KB + A_lo 8 KB
+constexpr int WG_NST = 3;                                       // shared-memory stages (operands are requested two k-blocks ahead)
+constexpr int WG_SMEM = WG_NST * WG_STAGE + 1024;               // + slack for 1024 B alignment
 
-VV_DEVINL unsigned long long umma_desc_sw128(unsigned smem_addr) {
-  return (unsigned long long)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// shared-memory matrix descriptor of a K-major bf16 operand with 128-byte swizzle: start address, leading byte offset (unused for this
+// layout, 16 B), stride byte offset 1024 B (one 8-row atom), layout type 1 = SWIZZLE_128B.  A k-step of 16 elements (32 B) inside the
+// atom is +2 on the start-address field; 64 rows further is +512.
+VV_DEVINL unsigned long long wgmma_desc_sw128(unsigned smem_addr) {
+  return (unsigned long long)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-VV_DEVINL void tc5_mma(unsigned tmem_d, unsigned long long adesc, unsigned long long bdesc, unsigned idesc, unsigned accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+VV_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+VV_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N_> VV_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N_) : "memory"); }
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory.  Accumulator fragment: register i of thread
+// (warp w of the warpgroup, lane l) holds row 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1).
+VV_DEVINL void wgmma_m64n16(float (&d)[8], unsigned long long a, unsigned long long b, int accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(a), "l"(b), "r"(accumulate) : "memory");
 }
-VV_DEVINL void tc5_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+VV_DEVINL void wgmma_m64n32(float (&d)[16], unsigned long long a, unsigned long long b, int accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(a), "l"(b), "r"(accumulate) : "memory");
+}
+VV_DEVINL void wgmma_m64n64(float (&d)[32], unsigned long long a, unsigned long long b, int accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(a), "l"(b), "r"(accumulate) : "memory");
 }
 
 // fp32 activations [M, K] (RowMap) -> dense bf16 planes hi, lo [M, K] with x = hi + lo (|err| <= 2^-17 |x|)
@@ -707,54 +722,42 @@ __global__ void split_bf16_kernel(const float* __restrict__ x, RowMap xmap, bf16
   }
 }
 
-__global__ void __launch_bounds__(128) gemm_tc5_kernel(GemvP p, const bf16* __restrict__ a_hi, const bf16* __restrict__ a_lo) {
-  extern __shared__ unsigned char t5_raw[];
-  __shared__ unsigned long long mma_bar[T5_NST];
-  __shared__ unsigned tmem_base_s;
-  const unsigned raw_addr = smem_u32(t5_raw);
-  unsigned char* sm = t5_raw + ((1024u - (raw_addr & 1023u)) & 1023u);      // 1024 B aligned (swizzle atom)
+__global__ void __launch_bounds__(128) gemm_wgmma_kernel(GemvP p, const bf16* __restrict__ a_hi, const bf16* __restrict__ a_lo) {
+  extern __shared__ unsigned char wg_raw[];
+  const unsigned raw_addr = smem_u32(wg_raw);
+  unsigned char* sm = wg_raw + ((1024u - (raw_addr & 1023u)) & 1023u);      // 1024 B aligned (swizzle atom)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int bn = blockIdx.x * T5_BM;       // weight rows (output features) of this CTA
-  const int bm = blockIdx.y * T5_BN;       // activation rows
-  const int K = p.K, nk = (K + T5_BK - 1) / T5_BK;
-
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"((unsigned)T5_BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 0) {
-    for (int i = 0; i < T5_NST; ++i) mbar_init(&mma_bar[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tmem_d = tmem_base_s;
+  const int bn = blockIdx.x * WG_BM;       // weight rows (output features) of this CTA
+  const int bm = blockIdx.y * WG_BN;       // activation rows
+  const int K = p.K, nk = (K + WG_BK - 1) / WG_BK;
 
   // one stage = W tile [128 x 64] + A_hi [64 x 64] + A_lo [64 x 64], all bf16, rows of 128 B, 16-byte chunks XOR-swizzled by (row & 7)
   auto load_w = [&](int stage, int kb) {   // 128 rows x 8 chunks: 8 cp.async per thread
-    unsigned char* wt = sm + stage * T5_STAGE;
+    unsigned char* wt = sm + stage * WG_STAGE;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int idx = tid + i * 128, r = idx >> 3, c = idx & 7;
-      const int n = bn + r, k = kb * T5_BK + c * 8;
+      const int n = bn + r, k = kb * WG_BK + c * 8;
       const bool ok = (n < p.N) && (k < K);
       cp_async16(wt + r * 128 + ((c ^ (r & 7)) << 4), p.W + (size_t)(ok ? n : 0) * K + (ok ? k : 0), ok ? 16 : 0);
     }
   };
   auto load_a = [&](int stage, int kb) {   // 2 planes x 64 rows x 8 chunks: 8 cp.async per thread
-    unsigned char* ah = sm + stage * T5_STAGE + T5_BM * 128;
+    unsigned char* ah = sm + stage * WG_STAGE + WG_BM * 128;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int idx = tid + i * 128, pl = idx >> 9, r = (idx >> 3) & 63, c = idx & 7;
-      const int m = bm + r, k = kb * T5_BK + c * 8;
+      const int m = bm + r, k = kb * WG_BK + c * 8;
       const bool ok = (m < p.M) && (k < K);
       const bf16* src = (pl ? a_lo : a_hi) + (size_t)(ok ? m : 0) * K + (ok ? k : 0);
-      cp_async16(ah + pl * (T5_BN * 128) + r * 128 + ((c ^ (r & 7)) << 4), src, ok ? 16 : 0);
+      cp_async16(ah + pl * (WG_BN * 128) + r * 128 + ((c ^ (r & 7)) << 4), src, ok ? 16 : 0);
     }
   };
-  // instruction descriptor: D=f32, A=B=bf16, both K-major, N=64, M=128
-  const unsigned idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(T5_BN >> 3) << 17) | ((unsigned)(T5_BM >> 4) << 24);
+  float acc[2][32];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
 
   pdl_trigger();
   load_w(0, 0);                                       // weights never depend on the predecessor grid
@@ -765,49 +768,48 @@ __global__ void __launch_bounds__(128) gemm_tc5_kernel(GemvP p, const bf16* __re
   if (nk > 1) load_a(1, 1);
   cp_async_commit();                                   // group 1 = A(1)
   for (int kb = 0; kb < nk; ++kb) {
-    const int st = kb % T5_NST;
-    cp_async_wait<1>();                                                 // everything of k-block kb has landed
+    const int st = kb % WG_NST;
+    cp_async_wait<1>();                                                 // this thread's copies of k-block kb have landed
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const unsigned wbase = smem_u32(sm + st * T5_STAGE);
-      const unsigned long long dw = umma_desc_sw128(wbase), dh = umma_desc_sw128(wbase + T5_BM * 128), dl = umma_desc_sw128(wbase + T5_BM * 128 + T5_BN * 128);
+    __syncthreads();                                                    // ... and everyone's
+    const unsigned wbase = smem_u32(sm + st * WG_STAGE);
+    const unsigned long long dw = wgmma_desc_sw128(wbase), dh = wgmma_desc_sw128(wbase + WG_BM * 128),
+                             dl = wgmma_desc_sw128(wbase + WG_BM * 128 + WG_BN * 128);
+    wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < T5_BK / 16; ++k) {               // UMMA_K = 16 bf16 = 32 B -> +2 in the 16-byte start-address field
-        tc5_mma(tmem_d, dw + 2 * k, dh + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-        tc5_mma(tmem_d, dw + 2 * k, dl + 2 * k, idesc, 1u);
+    for (int k = 0; k < WG_BK / 16; ++k) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        wgmma_m64n64(acc[h], dw + 512 * h + 2 * k, dh + 2 * k, 1);
+        wgmma_m64n64(acc[h], dw + 512 * h + 2 * k, dl + 2 * k, 1);
       }
-      tc5_commit(&mma_bar[st]);
     }
+    wgmma_commit();
     if (kb + 2 < nk) {
-      if (kb >= 1) mbar_wait(&mma_bar[(kb - 1) % T5_NST], (unsigned)(((kb - 1) / T5_NST) & 1));   // MMA(kb-1) released stage (kb+2)%3
-      load_w((kb + 2) % T5_NST, kb + 2);
-      load_a((kb + 2) % T5_NST, kb + 2);
+      wgmma_wait<1>();                     // this thread's MMAs of k-block kb-1 are done ...
+      __syncthreads();                     // ... and every warp's: stage (kb+2)%3 == (kb-1)%3 may be refilled
+      load_w((kb + 2) % WG_NST, kb + 2);
+      load_a((kb + 2) % WG_NST, kb + 2);
     }
     cp_async_commit();
   }
-  mbar_wait(&mma_bar[(nk - 1) % T5_NST], (unsigned)(((nk - 1) / T5_NST) & 1));
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  // epilogue: warp w owns TMEM lanes [32w, 32w+32) = weight rows n; columns = activation rows m
-  const int n = bn + warp * 32 + lane;
-  const float bias = (p.bias && n < p.N) ? p.bias[n] : 0.f;
+  wgmma_wait<0>();
+  // epilogue: rows of the fragment = weight rows n, columns = activation rows m
 #pragma unroll
-  for (int c0 = 0; c0 < T5_BN; c0 += 8) {
-    unsigned r[8];
-    const unsigned taddr = tmem_d + ((unsigned)(warp * 32) << 16) + (unsigned)c0;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int m = bm + c0 + j;
-      if (m < p.M && n < p.N) epi_store(p, m, n, __uint_as_float(r[j]) + bias);
+    for (int e = 0; e < 2; ++e) {
+      const int n = bn + h * 64 + warp * 16 + (lane >> 2) + 8 * e;
+      if (n >= p.N) continue;
+      const float bias = p.bias ? p.bias[n] : 0.f;
+#pragma unroll
+      for (int j = 0; j < WG_BN / 8; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int m = bm + 8 * j + 2 * (lane & 3) + c;
+          if (m < p.M) epi_store(p, m, n, acc[h][4 * j + 2 * e + c] + bias);
+        }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((unsigned)T5_BN) : "memory");
 }
 
 // thread-per-output small-K product with fp32 weights (encoder stem conv 1->32 k7, decoder head conv 32->1 k7)

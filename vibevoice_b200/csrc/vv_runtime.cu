@@ -89,8 +89,8 @@ struct vv_ctx {
   bool use_splitk = true;
   bool fuse_rope = true;
   bf16* s_planes = nullptr; size_t planes_elems = 0;
-  int mma_min_rows = 9;     // M >= this -> tensor-core GEMM (all prologues/epilogues), below -> weight-streaming GEMV (measured: at M = 8 the GEMV streams weights 1.7x faster)
-  int use_tc5 = 1;          // tcgen05/TMEM GEMM: 0 off, 1 auto (wide GEMMs), 2 every M > 8 GEMM (VV_TC5)
+  int mma_min_rows = 9;     // M >= this -> tensor-core GEMM (all prologues/epilogues), below -> weight-streaming GEMV (at M = 8 the GEMV streams weights faster)
+  int use_wgmma = 1;        // warpgroup (wgmma) GEMM: 0 off, 1 auto (wide GEMMs), 2 every M > 8 GEMM (VV_WGMMA)
   bool ring_rms = true;     // RMSNorm folded into gemm_mma_ring_kernel (row scale in the epilogue) instead of rows_norm_kernel (VV_NO_RING_RMS=1 -> off)
   int codec_mma_min_rows = 9;   // codec GEMMs with at least this many rows use the tensor-core ring kernel (VV_CODEC_MMA_MIN_ROWS)
   bool mma_ring = true;     // 6-stage cp.async ring for both GEMM operands (gemm_mma_ring_kernel); VV_NO_MMA_RING=1 -> old 1-ahead kernel
@@ -98,7 +98,7 @@ struct vv_ctx {
   int wr_tasks_min = 296;
   int wr_force = 0;
   int gemv_grid_cap = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   std::map<std::string, RawTensor> raw;
   std::set<std::string> expected;
   std::vector<void*> allocs;
@@ -228,17 +228,17 @@ static int gemv_occupancy(vv_ctx* c, int smem) {
 static int linear(const L& l, GemvP p) {
   if (p.K % 8 != 0) return fail(VV_ERR_INVALID, "linear: K=%d not a multiple of 8", p.K);
   if (((uintptr_t)p.x & 15) || (p.xmap.rs & 3) || (p.xmap.bs & 3)) return fail(VV_ERR_INVALID, "linear: activation rows must be 16-byte aligned");
-  // tcgen05/TMEM path: wide GEMMs that fill the chip with 128-row weight tiles (the all-steps AdaLN modulation GEMM:
+  // wgmma path: wide GEMMs that fill the chip with 128-row weight tiles (the all-steps AdaLN modulation GEMM:
   // [N_steps*2B, H] x [(3L+2)H, H]^T = 168 CTAs on 1.5B); mode 2 forces it for every M > 8 GEMM (tests)
-  const int tc5_ctas = ((p.N + T5_BM - 1) / T5_BM) * ((p.M + T5_BN - 1) / T5_BN);
-  if (l.c->use_tc5 && p.M > 8 && p.pro == PRO_NONE && p.epi != EPI_SWIGLU && (l.c->use_tc5 == 2 || tc5_ctas >= 96)) {
-    if ((size_t)p.M * p.K > l.c->planes_elems) return fail(VV_ERR_INVALID, "tc5: activation planes scratch too small (%d x %d)", p.M, p.K);
+  const int wg_ctas = ((p.N + WG_BM - 1) / WG_BM) * ((p.M + WG_BN - 1) / WG_BN);
+  if (l.c->use_wgmma && p.M > 8 && p.pro == PRO_NONE && p.epi != EPI_SWIGLU && (l.c->use_wgmma == 2 || wg_ctas >= 96)) {
+    if ((size_t)p.M * p.K > l.c->planes_elems) return fail(VV_ERR_INVALID, "wgmma: activation planes scratch too small (%d x %d)", p.M, p.K);
     bf16* hi = l.c->s_planes;
     bf16* lo = l.c->s_planes + l.c->planes_elems;
     const long long n4 = (long long)p.M * (p.K >> 2);
     CK(launch_k(l, split_bf16_kernel, dim3((unsigned)std::min<long long>((n4 + 255) / 256, 1184)), dim3(256), 0, p.x, p.xmap, hi, lo, p.M, p.K));
-    CK(cudaFuncSetAttribute(gemm_tc5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T5_SMEM));
-    CK(launch_k(l, gemm_tc5_kernel, dim3((p.N + T5_BM - 1) / T5_BM, (p.M + T5_BN - 1) / T5_BN), dim3(128), (size_t)T5_SMEM, p, (const bf16*)hi, (const bf16*)lo));
+    CK(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+    CK(launch_k(l, gemm_wgmma_kernel, dim3((p.N + WG_BM - 1) / WG_BM, (p.M + WG_BN - 1) / WG_BN), dim3(128), (size_t)WG_SMEM, p, (const bf16*)hi, (const bf16*)lo));
     return 0;
   }
   if (p.M >= l.c->mma_min_rows) {
@@ -340,7 +340,7 @@ static int tiled_weight(vv_ctx* c, const bf16* W, int N, int K, bool fresh, bf16
   bf16* T = nullptr;
   RET(dmalloc(c, &T, (size_t)(*n_tiles) * 8192, false));
   const long long n_chunks = *n_tiles * 1024;
-  tile_pack_kernel<<<(unsigned)std::min<long long>((n_chunks + 255) / 256, 148 * 32), 256>>>(W, T, N, K, (int)KB, n_chunks);
+  tile_pack_kernel<<<(unsigned)std::min<long long>((n_chunks + 255) / 256, (long long)c->sm_count * 32), 256>>>(W, T, N, K, (int)KB, n_chunks);
   CKL();
   CK(cudaDeviceSynchronize());
   if (!fresh) c->tiled[W] = T;
@@ -467,7 +467,7 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
     const long long count = std::min(per, KB);
     b_bytes = std::max<long long>(b_bytes, count * o.nB * 128);
     const long long segs = (per + KB - 1) / KB + 1;
-    if (segs > ST_MAXSEG || segs * o.nB > 512) return fail(VV_ERR_INVALID, "stream: stage [%d x %d] needs %lld accumulators per CTA", o.N, o.K, segs);
+    if (segs > ST_MAXSEG) return fail(VV_ERR_INVALID, "stream: stage [%d x %d] needs %lld accumulators per CTA", o.N, o.K, segs);
     if (o.store && KB != 1) return fail(VV_ERR_INVALID, "stream: store epilogue needs K <= 64");
     if (o.pro == SP_WINDOW && (o.cod.cin % 8)) return fail(VV_ERR_INVALID, "stream: window prologue needs a channel count that is a multiple of 8");
     if (o.pro == SP_COMBINE) {
@@ -616,14 +616,14 @@ extern "C" int vv_create(const vv_model_desc* desc, int device, vv_ctx** out) {
   c->use_graphs = !(ng && ng[0] == '1');
   const char* na = getenv("VV_SCALAR_ATTN");
   c->use_mma_attn = !(na && na[0] == '1');
-  c->wr_tasks_min = c->sm_count;      // measured (tools/bench_gemv.py): one task per SM beats two for the N=1536 shapes, neutral elsewhere
+  c->wr_tasks_min = c->sm_count;      // one task per SM (tools/bench_gemv.py compares geometries)
   if (getenv("VV_WR_TASKS_MIN")) c->wr_tasks_min = atoi(getenv("VV_WR_TASKS_MIN"));
   if (getenv("VV_WR_FORCE")) c->wr_force = atoi(getenv("VV_WR_FORCE"));
   if (getenv("VV_GEMV_GRID_CAP")) c->gemv_grid_cap = atoi(getenv("VV_GEMV_GRID_CAP"));
   if (getenv("VV_NO_FUSE_ROPE")) c->fuse_rope = false;
   if (getenv("VV_STREAM")) c->use_stream = atoi(getenv("VV_STREAM"));
   if (getenv("VV_STREAM_INFLIGHT")) c->st_inflight = atoi(getenv("VV_STREAM_INFLIGHT"));
-  if (getenv("VV_TC5")) c->use_tc5 = atoi(getenv("VV_TC5"));
+  if (getenv("VV_WGMMA")) c->use_wgmma = atoi(getenv("VV_WGMMA"));
   if (getenv("VV_MMA_MIN_ROWS")) c->mma_min_rows = atoi(getenv("VV_MMA_MIN_ROWS"));
   if (getenv("VV_NO_MMA_RING")) c->mma_ring = false;
   if (getenv("VV_NO_RING_RMS")) c->ring_rms = false;
@@ -948,7 +948,7 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
       int maxp = 0, maxw = 0;
       cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, c->device);
       cudaDeviceGetAttribute(&maxw, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
-      size_t want = 0;     // measured neutral on B200 (79 MB max set-aside, sampler is latency- not bandwidth-bound): opt-in via VV_L2_PERSIST_MB
+      size_t want = 0;     // off by default (the sampler is latency- rather than bandwidth-bound): opt-in via VV_L2_PERSIST_MB
       if (getenv("VV_L2_PERSIST_MB")) want = (size_t)atoi(getenv("VV_L2_PERSIST_MB")) << 20;
       c->l2_persist_bytes = std::min<size_t>(want, (size_t)maxp);
       c->l2_window_max = (size_t)maxw;
@@ -1754,7 +1754,7 @@ static int enqueue_block(const L& l, const Block& b, const float* xin, float* xo
     CK(launch_k(l, dwconv_res_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, xin, c->s_win, b.dw_w, b.dw_b, b.gamma, xout, B, T, C));
   }
   GemvP p;
-  if (M < c->mma_min_rows || (c->ring_rms && c->mma_ring && C <= MR_MAXK_NORM && c->use_tc5 != 2)) {
+  if (M < c->mma_min_rows || (c->ring_rms && c->mma_ring && C <= MR_MAXK_NORM && c->use_wgmma != 2)) {
     p = mk(b.w1, b.b1, xout, C, c->s_u, 4 * C, M, 4 * C, C);
     p.pro = PRO_RMSNORM; p.pro_w = b.ffn_norm_w; p.pro_eps = eps; p.epi = EPI_GELU;
     RET(linear(l, p));
@@ -2162,28 +2162,6 @@ extern "C" int vv_stream_trace_read(vv_ctx* c, long long* out, int* out_meta, in
     break;
   }
   return n;
-}
-// tcgen05.mma 128 x nB x 16 rate micro-benchmark (vv_stream.cuh: mma_rate_kernel); cycles_out = median over CTAs of the loop's SM cycles
-extern "C" int vv_debug_mma_rate(vv_ctx* c, int n, int nB, int mode, int nacc, int ctas, long long* cycles_out) {
-  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  CK(cudaSetDevice(c->device));
-  if (nacc < 1 || nacc * nB > 512 || nB > 256) return fail(VV_ERR_INVALID, "nacc * nB must be <= 512, nB <= 256");
-  long long* d = nullptr;
-  CK(cudaMalloc(&d, sizeof(long long) * 2 * ctas));
-  CK(cudaMemset(d, 0, sizeof(long long) * 2 * ctas));
-  const int smem = 8 * ST_TILE + 32768 + 1024;
-  CK(cudaFuncSetAttribute(mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  mma_rate_kernel<<<ctas, 128, smem>>>(n, nB, mode, nacc, d);
-  CKL();
-  CK(cudaDeviceSynchronize());
-  std::vector<long long> h(2 * ctas);
-  CK(cudaMemcpy(h.data(), d, sizeof(long long) * 2 * ctas, cudaMemcpyDeviceToHost));
-  cudaFree(d);
-  std::sort(h.begin(), h.begin() + ctas);
-  std::sort(h.begin() + ctas, h.end());
-  cycles_out[0] = h[ctas / 2];              // whole loop incl. completion
-  cycles_out[1] = h[ctas + ctas / 2];       // issue loop only
-  return 0;
 }
 // watchdog record of the last stream kernel that trapped: out[0] = code (0 = none), out[1..5] = cta, thread, stage, iteration, extra
 extern "C" int vv_stream_diag(vv_ctx* c, unsigned* out6) {

@@ -1,24 +1,25 @@
-// vv_stream.cuh -- persistent weight-stream kernel: every M <= 8..64-row linear of the generation loop as a tcgen05 / TMEM MMA whose
+// vv_stream.cuh -- persistent weight-stream kernel: every M <= 8..64-row linear of the generation loop as a warpgroup MMA (wgmma) whose
 // weight tiles arrive by TMA (cp.async.bulk.tensor, 128-byte swizzle) through a deep shared-memory ring that keeps running ACROSS the
 // grid-wide dependencies between stages.
 //
-// Why this shape (profiles/r01_*, DESIGN 7): one speech frame is a chain of ~450 dependent skinny linears (28 LM layers x 4, 30 diffusion
-// steps x 9, codec front).  As one kernel per stage each of them pays launch + cold pipeline + drain (~5 us) around a 1-9 us weight
-// stream, and HBM idles in between: 0.33 of the roofline.  Here ONE cooperative grid (one CTA per SM) runs a whole program of stages:
+// Why this shape (DESIGN 7): one speech frame is a chain of ~450 dependent skinny linears (28 LM layers x 4, 30 diffusion steps x 9,
+// codec front).  As one kernel per stage each of them pays launch + cold pipeline + drain (~5 us) around a 1-9 us weight stream, and HBM
+// idles in between.  Here ONE cooperative grid (one CTA per SM) runs a whole program of stages:
 //
-//   warp 0   producer   walks the program's static schedule and issues the TMA loads of this CTA's weight tiles (128 rows x 64 k, bf16,
+//   warps 0-3 workers   (one warpgroup) grid barrier -> prologue: activations from L2, RMSNorm / AdaLN / SwiGLU / GELU / solver update
+//                       applied, split into bf16 hi + lo (x = hi + lo to 2^-17) and written as the MMA's B operand in the canonical K-major
+//                       SWIZZLE_128B layout (rows [0, nB/2) = hi, [nB/2, nB) = lo, so ONE MMA yields both partial products) -> per weight
+//                       tile 2 x 4 wgmma.mma_async m64 x nB x 16 (the tile's two 64-row halves, N = 16..64 activation rows), fp32
+//                       accumulators in registers, the ring slot handed back to the producer once its MMAs retired -> epilogue per
+//                       (row tile, k range) segment straight from the accumulators: hi + lo, bias / gate / gamma scaling, fp32 atomics
+//                       (red.global.add) into the output.
+//   warp 4   producer   walks the program's static schedule and issues the TMA loads of this CTA's weight tiles (128 rows x 64 k, bf16,
 //                       16 KB) into an S-stage ring.  Weights never depend on activations, so it runs ahead of the grid barriers: while
-//                       the other warps synchronise / stage activations for stage i, the ring already fills with tiles of stage i, i+1...
-//   warp 1   MMA        one elected thread: per tile 4 x tcgen05.mma.cta_group::1.kind::f16 (M = 128 weight rows, N = 16..64 activation
-//                       rows, K = 16), fp32 accumulators in TMEM; tcgen05.commit hands the ring slot back to the producer.
-//   warps 2-5 workers   grid barrier -> prologue: activations from L2, RMSNorm / AdaLN / SwiGLU / GELU / solver update applied, split into
-//                       bf16 hi + lo (x = hi + lo to 2^-17) and written as the MMA's B operand in the canonical K-major SWIZZLE_128B
-//                       layout (rows [0, nB/2) = hi, [nB/2, nB) = lo, so ONE MMA yields both partial products) -> epilogue: tcgen05.ld
-//                       of the accumulators, hi + lo, bias / gate / gamma scaling, fp32 atomics (red.global.add) into the output.
+//                       the workers synchronise / stage activations for stage i, the ring already fills with tiles of stage i, i+1...
 //
 // Work split ("stream-K"): a stage with R = ceil(N/128) row tiles and KB = ceil(K/64) k-blocks has U = R*KB tile units, dealt out as
 // contiguous ranges [c*U/G, (c+1)*U/G) to the G CTAs in row-tile-major order: every SM streams the same number of bytes (+-1 tile) for
-// ANY shape, a CTA owns <= 3 (row tile, k range) segments, each with its own TMEM accumulator, and partial sums meet in the output through
+// ANY shape, a CTA owns <= 3 (row tile, k range) segments, each accumulated and written out in turn, and partial sums meet in the output through
 // atomics.  That is why epilogues are linear (bias, scaling, residual) and the non-linearities (SwiGLU, GELU) live in the NEXT stage's
 // prologue.
 //
@@ -26,8 +27,7 @@
 // RoPE / KV append fused, split-KV partials merged in the o-projection's prologue.  Codec stages add a causal-window gather prologue and a
 // distributed mixer stage (SK_MIX).
 //
-// What the round's measurements say about this kernel (DESIGN 3.1 / 8, profiles/r02_*): DRAM bytes = algorithmic bytes, DRAM ~30 % busy, tensor
-// pipe < 5 % -- it is bound by the chain of ~520 dependent grid-wide stages per frame, and INSIDE a stage by instruction fetch: every stage runs
+// The kernel is bound by the chain of ~520 dependent grid-wide stages per frame, and INSIDE a stage by instruction fetch: every stage runs
 // its worker path once, straight-line.  Hence one instantiation per program family (stream_kernel<FEAT, TRACE>), compile-time head_dim / operand
 // height where a program allows it, descriptor fields in registers, descriptor-only arithmetic between barrier arrival and barrier wait, and
 // uniform early exits instead of predicated-off rows.
@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(256) barrier_bench_kernel(GridBar* gb, int ite
 // ---------------------------------------------------------------------------------------------------------------------------------
 // program representation (built on the host in vv_runtime.cu, read-only on the device)
 // ---------------------------------------------------------------------------------------------------------------------------------
-constexpr int ST_THREADS = 192;          // warp 0 producer, warp 1 MMA issuer, warps 2..5 workers
+constexpr int ST_THREADS = 160;          // warps 0..3 workers (one warpgroup: wgmma), warp 4 producer
 constexpr int ST_WORKERS = 128;
 constexpr int ST_TILE = 16384;           // one weight tile: 128 rows x 64 bf16
 constexpr int ST_MAXSEG = 8;             // (row tile, k range) segments a CTA may own in one stage
@@ -127,7 +127,7 @@ struct SAtt {
   unsigned row_base;           // first row of this layer in those maps
   int hd;                      // head_dim: 128 (a K / V page = two 64-column boxes) or 64 (one box, 8 KB of the slot used)
   float* rope_cs;              // [M][64][2] cos / sin of (kv_len[m] * inv_freq[d]): written by the QKV stage, read here (accurate sincosf of
-                               // positions up to 64K costs ~1 us per segment when every CTA recomputes it)
+                               // positions up to 64K is too slow to recompute in every CTA)
 };
 
 // Streaming-codec prologues (modular_vibevoice_tokenizer.py:327-382, 620-684; same arithmetic as assemble_window / dwconv_res / rows_norm):
@@ -137,7 +137,7 @@ struct SAtt {
 //  SK_MIX     (a stage of its own, no linear) the first half of a Block1D for rows (b, t), t < T, C = K channels, channels dealt out to CTAs:
 //             xn = RMSNorm(x) * norm_w;  x1 = x + gamma * (dw_b + sum_j dw_w[j] * win[t + j]),  win = [hist[b] (6 normalised rows) ; xn];
 //             writes x1 (the residual base both FFN linears work on) and the next history (last 6 rows of the window).
-//             (Tried first as the prologue of the FFN linear, recomputed by every CTA: 14-30 us per block, profiles/r02_stream_trace_codec_1.txt.)
+//             (As the prologue of the FFN linear every CTA would recompute the whole block's mixer.)
 struct SCodec {
   const float* hist; float* next;        // [B][ctx][cin] / [B][6][C]
   const float* src;                      // SP_WINDOW: [B][T_in][cin]
@@ -184,11 +184,10 @@ struct SParams {
   long long* trace2;        // optional [n_ops][G][2] globaltimer (ns) of every CTA: arrival at / release from the grid barrier
 };
 constexpr int ST_TRACE = 12;   // 0 op start, 1 barrier passed, 2 row stats done, 3 B operand staged, 4 accumulators complete, 5 epilogue issued,
-                               // 6 MMA saw b_ready, 7 MMA saw the last tile, 8 MMA committed, 9 producer issued the last tile of the stage
+                               // 6 MMA loop entered, 7 MMA saw the last tile, 8 last MMA retired, 9 producer issued the last tile of the stage
 
-// W [N][K] row-major -> tile-major [R][KB][128][64], zero padded.  Measured (profiles/r02_stream_trace_1.txt): TMA boxes cut out of the
-// row-major matrix (128 rows x 128 B, 3 KB apart) stream at 2.4 TB/s -- every row is its own DRAM burst -- so the kernel reads tiles that are
-// contiguous in HBM instead; units of a stage are consecutive tiles, i.e. every CTA reads ONE contiguous byte range per stage.
+// W [N][K] row-major -> tile-major [R][KB][128][64], zero padded.  TMA boxes cut out of the row-major matrix (128 rows x 128 B, kilobytes
+// apart) make every row its own DRAM burst, so the kernel reads tiles that are contiguous in HBM instead; units of a stage are consecutive tiles, i.e. every CTA reads ONE contiguous byte range per stage.
 __global__ void tile_pack_kernel(const bf16* __restrict__ W, bf16* __restrict__ T, int N, int K, int KB, long long n_chunks) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_chunks; i += (long long)gridDim.x * blockDim.x) {
     const int ch = (int)(i & 7), r = (int)((i >> 3) & 127);
@@ -241,17 +240,14 @@ VV_DEVINL void worker_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 // attention units of row m: kv_heads * pages(m) (0 for rows that are switched off); returns the total, fills this CTA's range
 // kv_len / row_mode are constant during a launch; the kernel keeps a copy in shared memory (SeqView) -- read from global memory at the start
-// of every attention stage they were 4 dependent L2 round trips, ~2.5 us, on the critical path
+// of every attention stage they were 4 dependent L2 round trips on the critical path
 struct SeqView { const int* kv_len; const int* row_mode; int kv_heads; };
 VV_DEVINL unsigned att_tiles(const SeqView& q, int m) { return q.row_mode[m] ? (unsigned)((q.kv_len[m] + 1 + KV_PAGE - 1) / KV_PAGE) : 0u; }
 // Work split of an attention stage.  Every (row m, kv head g) group with pages contributes nt + ST_ATT_SEGW VIRTUAL units: the first
-// ST_ATT_SEGW stand for the fixed cost of a segment (Q staging, warp merge, partial write ~ 3.6 us ~ 4 pages), the rest are its pages in
+// ST_ATT_SEGW stand for the fixed cost of a segment (Q staging, warp merge, partial write ~ 4 pages), the rest are its pages in
 // order.  CTAs take contiguous ranges of virtual units, so a CTA that also gets the few pages of a short (CFG-negative) row gets
-// correspondingly fewer pages of the long one (measured before: the CTA owning both short groups arrived 8 us late at every layer's barrier).
+// correspondingly fewer pages of the long one (otherwise the CTA owning both short groups arrives late at every layer's barrier).
 constexpr unsigned ST_ATT_SEGW = 4;
-// Tried and measured on one box, then removed again (profiles/r02_ab_wide_inflight.txt, r02_ab_gate_prefetch_trace_offsets.txt): four activation
-// chunks per thread in one L2 round trip (LM -0.5 %, sampler +4.7 %: 1 900 more instructions), swizzled B-operand offsets precomputed ahead of the
-// barrier (+0.5 %), epilogue-operand prefetch that stops at the last live segment (no gain).
 VV_DEVINL unsigned att_vtotal(const SeqView& q, int M) {
   unsigned V = 0;
   for (int m = 0; m < M; ++m) { const unsigned nt = att_tiles(q, m); if (nt) V += (nt + ST_ATT_SEGW) * (unsigned)q.kv_heads; }
@@ -285,7 +281,7 @@ VV_DEVINL bool att_next(const SeqView& q, int M, AttIter& it, AttSeg& sg) {
 VV_DEVINL unsigned kv_off(int tok, int d) { return (unsigned)(((d >> 6) << 13) + tok * 128 + ((((d & 63) >> 3) ^ (tok & 7)) << 4) + (d & 7) * 2); }
 
 // this CTA's unit range of a stage: units are (row tile, k-block) pairs in row-tile-major order
-// (32-bit arithmetic: U * gridDim < 2^32 is checked on the host; 64-bit divisions here cost ~0.3 us per stage on the critical path)
+// (32-bit arithmetic: U * gridDim < 2^32 is checked on the host; 64-bit divisions here would sit on the critical path of every stage)
 VV_DEVINL void st_part(const SOp& op, unsigned& u0, unsigned& u1, int& KB) {
   KB = (op.K + 63) >> 6;
   const unsigned U = (unsigned)((op.N + 127) >> 7) * (unsigned)KB;
@@ -293,12 +289,112 @@ VV_DEVINL void st_part(const SOp& op, unsigned& u0, unsigned& u1, int& KB) {
   u1 = U * (blockIdx.x + 1u) / gridDim.x;
 }
 
+// epilogue operands of a linear stage: y[m][n] (+)= alpha * (acc + bias[n] if the segment starts at k = 0)
+struct StEpi { const float* bias; const float* alpha; float* y; long long lda, ldy; bool gate, gamma, store; };
+
+template <int NB> VV_DEVINL void wgmma_nb(float (&d)[NB / 2], unsigned long long a, unsigned long long b) {
+  if constexpr (NB == 16) wgmma_m64n16(d, a, b, 1);
+  else if constexpr (NB == 32) wgmma_m64n32(d, a, b, 1);
+  else wgmma_m64n64(d, a, b, 1);
+}
+
+// The worker warpgroup's MMA + epilogue of one linear stage: units [u0, u1) = (row tile, k-block) pairs whose weight tiles sit in the ring
+// from slot `slot` (phase `ph`) on, B operand of k-block j (relative to the first one) at breg + j * NB * 128.  The units form <= 3
+// (row tile, k range) segments.  Per segment: the epilogue operands (bias, gamma, gate) are requested first, so they arrive while the MMAs
+// run; per tile the two 64-row halves of the weight tile times the NB-row operand, 4 k-steps each, the MMAs of a tile running while the
+// next tile's are issued and its ring slot released once they retired; then the accumulators go out through the epilogue.
+template <int NB>
+VV_DEVINL void st_mma_epilogue(unsigned char* ring, unsigned char* breg, unsigned long long* full_bar, unsigned long long* empty_bar, int NS,
+                               unsigned slot, unsigned ph, unsigned u0, unsigned u1, int KB, int M, int N, const StEpi& ep, unsigned* diag,
+                               int oi, long long* trs) {
+  constexpr int R = NB / 2;                  // accumulator registers per 64-row half; operand rows [0, NB/2) = hi, [NB/2, NB) = lo
+  constexpr int HG = NB / 16;                // 8-column groups of the hi half
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned long long da0 = wgmma_desc_sw128(smem_u32(ring)), db0 = wgmma_desc_sw128(smem_u32(breg));
+  const unsigned bstep = (unsigned)(NB * 128) >> 4;          // descriptor start-address units (16 B) per k-block of the B operand
+  const int rt_first = (int)(u0 / (unsigned)KB), kb_first = (int)(u0 - (unsigned)rt_first * (unsigned)KB);
+  if (trs) trs[6] = clock64();
+  unsigned jloc = 0;
+  int rt = rt_first, kb = kb_first;
+  for (unsigned u = u0; u < u1; ++rt, kb = 0) {
+    const unsigned seg_end = min(u1, u + (unsigned)(KB - kb));
+    // ---------------- epilogue operands of row tile rt: requested now, consumed after the MMAs ----------------
+    const bool from0 = kb == 0;                               // this segment holds k-block 0 of its row tile -> it adds the bias
+    float e_bias[2][2], e_gam[2][2], e_gate[2][2][HG][2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = rt * 128 + h * 64 + warp * 16 + (lane >> 2) + 8 * e;
+        const bool live = n < N;
+        e_bias[h][e] = (live && from0 && ep.bias) ? ep.bias[n] : 0.f;
+        e_gam[h][e] = (live && ep.gamma) ? ep.alpha[n] : 1.f;
+#pragma unroll
+        for (int j = 0; j < HG; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int m = 8 * j + 2 * (lane & 3) + c;
+            e_gate[h][e][j][c] = (live && ep.gate && m < M) ? ldcg1(ep.alpha + (long long)m * ep.lda + n) : 1.f;
+          }
+      }
+    // ---------------- MMAs of the segment ----------------
+    float acc[2][R];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < R; ++i) acc[h][i] = 0.f;
+    unsigned prev = 0;
+    for (unsigned v = u; v < seg_end; ++v) {
+      mbar_wait_wd(&full_bar[slot], ph, diag, 3u, (unsigned)oi, v - u0);
+      __syncwarp();                                           // reconverge after the per-thread spin: wgmma is warpgroup-collective
+      if (trs && v + 1 == u1) trs[7] = clock64();
+      const unsigned long long da = da0 + (unsigned long long)(slot * (unsigned)(ST_TILE >> 4));
+      const unsigned long long db = db0 + (unsigned long long)(jloc * bstep);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        wgmma_nb<NB>(acc[0], da + 2 * k, db + 2 * k);
+        wgmma_nb<NB>(acc[1], da + 512 + 2 * k, db + 2 * k);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                        // this warp's MMAs of the previous tile retired: hand its slot back
+      if (v > u && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = slot;
+      if (++slot == (unsigned)NS) { slot = 0; ph ^= 1u; }
+      if (++jloc == (unsigned)KB) jloc = 0;                   // (only when the CTA holds >= KB units: B region = all k-blocks)
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (trs && seg_end == u1) { trs[4] = clock64(); trs[8] = trs[4]; }
+    u = seg_end;
+    // ---------------- epilogue of row tile rt ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = rt * 128 + h * 64 + warp * 16 + (lane >> 2) + 8 * e;
+        if (n >= N) continue;
+#pragma unroll
+        for (int j = 0; j < HG; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int m = 8 * j + 2 * (lane & 3) + c;
+            if (m < M) {
+              const float val = (acc[h][4 * j + 2 * e + c] + acc[h][4 * (j + HG) + 2 * e + c] + e_bias[h][e]) * e_gam[h][e] * e_gate[h][e][j][c];
+              float* yp = ep.y + (long long)m * ep.ldy + n;
+              if (ep.store) *yp = val; else red_add_f32(yp, val);
+            }
+          }
+      }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------------------------------------------
 // FEAT = the stage kinds / prologues / epilogue scalings a program may use (bit SP_x, bit 16 + SK_x, bit 24 + SA_x).  One instantiation per
 // program family: the all-features kernel is 224 KB of SASS and every stage runs its path exactly once, so the instruction cache misses
-// on most of it -- measured on one box (tools/ab_run.sh): +1 900 instructions of code a program never executes cost the sampler 4.7 %.
+// on most of it: code a program never executes costs time (compare instantiations with tools/ab_run.sh).
 // TRACE = per-stage clock stamps compiled in (tools/stream_trace.py); the production instantiations carry none of that code.
 template <unsigned FEAT, bool TRACE>
 __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
@@ -312,8 +408,6 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
 #define OP_NB(o) ((((FEAT >> 29) & 1u) != 0u) ? 16 : (o).nB)
   extern __shared__ unsigned char st_raw[];
   __shared__ unsigned long long full_bar[ST_MAX_STAGES], empty_bar[ST_MAX_STAGES];
-  __shared__ unsigned long long b_ready, acc_full;
-  __shared__ unsigned tmem_base_s;
   __shared__ float s_red[4][8];
   __shared__ float s_inv[64];
   __shared__ float s_z[8 * 64];
@@ -334,21 +428,13 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
   SeqView seq; seq.kv_len = s_kvlen; seq.row_mode = s_rmode; seq.kv_heads = P.kv_heads;
 
   if (tid == 0) {
-    for (int i = 0; i < NS; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(&b_ready, 1);
-    mbar_init(&acc_full, 1);
+    // a ring slot is free again when each of the four worker warps has seen its MMAs retire (or its attention reads end): 4 arrivals
+    for (int i = 0; i < NS; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], ST_WORKERS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tmem = tmem_base_s;
 
-  if (warp == 0) {
+  if (warp == ST_WORKERS / 32) {
     // =============================== producer: weights only, never waits on activations ===============================
     if (lane == 0) {
       unsigned long long policy;
@@ -410,87 +496,15 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
         if (TRACE && P.trace && (int)blockIdx.x == P.trace_cta) P.trace[(size_t)oi * ST_TRACE + 9] = clock64();
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    // The WHOLE warp runs this loop converged and one elected lane issues (elect.sync inside the asm block).  Measured
-    // (profiles/r02_mma_rate.txt): tcgen05.mma issued from `if (lane == 0)` with per-iteration operands costs 424 cycles per instruction
-    // (the compiler wraps UTCHMMA in a per-thread uniformisation loop), 84 from a converged warp, 46 with loop-invariant operands --
-    // at 4 MMAs per 16 KB tile the first form alone capped a CTA at HBM speed.
-    unsigned slot = 0, ph = 0, gi = 0;
-    for (int oi = 0; oi < P.n_ops; ++oi) {
-      const SOp& op = P.ops[oi];
-      if (KIND_IS(SK_ATTN)) {                                  // the workers consume 2 ring slots per attention unit: keep slot / phase in step
-        AttIter ai; AttSeg sg;
-        att_begin(seq, op.M, ai);
-        unsigned pages = 0;
-        while (att_next(seq, op.M, ai, sg)) pages += (unsigned)(sg.t1 - sg.t0);
-        const unsigned adv = 2u * pages + slot;
-        ph ^= (adv / (unsigned)NS) & 1u;
-        slot = adv % (unsigned)NS;
-        continue;
-      }
-      if (op.kind != SK_GEMV) continue;
-      unsigned u0, u1; int KB;
-      st_part(op, u0, u1, KB);
-      if (u0 == u1) continue;
-      const int nB = OP_NB(op);
-      // instruction descriptor: D = f32, A = B = bf16, both K-major, N = nB, M = 128
-      const unsigned idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(nB >> 3) << 17) | ((unsigned)(128 >> 4) << 24);
-      const int kb_first = (int)(u0 % (unsigned)KB);
-      const int units = (int)(u1 - u0);
-      const unsigned long long db0 = umma_desc_sw128(smem_u32(breg));
-      const unsigned long long da0 = umma_desc_sw128(smem_u32(ring));
-      const unsigned bstep = (unsigned)(nB * 128) >> 4;          // descriptor start-address units (16 B) per k-block of the B operand
-      mbar_wait_wd(&b_ready, gi & 1u, P.diag, 2u, (unsigned)oi, gi);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const bool tr = TRACE && P.trace && (int)blockIdx.x == P.trace_cta && lane == 0;
-      if (tr) P.trace[(size_t)oi * ST_TRACE + 6] = clock64();
-      int kb = kb_first;                                         // k-block of the current unit; jloc = position in the staged B region
-      unsigned jloc = 0, dcol = tmem, fresh = 1;
-      for (int ui = 0; ui < units; ++ui) {
-        mbar_wait_wd(&full_bar[slot], ph, P.diag, 3u, (unsigned)oi, (unsigned)ui);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const unsigned long long da = da0 + (unsigned long long)(slot * (unsigned)(ST_TILE >> 4));
-        const unsigned long long db = db0 + (unsigned long long)(jloc * bstep);
-        const unsigned ebar = smem_u32(&empty_bar[slot]);
-        asm volatile(
-            "{\n\t.reg .pred e, p, t;\n\t"
-            "elect.sync _|e, 0xffffffff;\n\t"
-            "setp.eq.b32 p, %5, 0;\n\t"
-            "setp.eq.b32 t, 0, 0;\n\t"
-            "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-            "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %6, %7, %3, t;\n\t"
-            "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %8, %9, %3, t;\n\t"
-            "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %10, %11, %3, t;\n\t"
-            "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%4];\n\t"
-            "}"
-            ::"r"(dcol), "l"(da), "l"(db), "r"(idesc), "r"(ebar), "r"(fresh),
-              "l"(da + 2), "l"(db + 2), "l"(da + 4), "l"(db + 4), "l"(da + 6), "l"(db + 6) : "memory");
-        fresh = 0;
-        if (++slot == (unsigned)NS) { slot = 0; ph ^= 1u; }
-        ++jloc;
-        if (++kb == KB) { kb = 0; dcol += (unsigned)nB; fresh = 1; }     // next row tile: its own accumulator, first MMA overwrites
-        if (jloc == (unsigned)KB) jloc = 0;                                // (only when the CTA holds >= KB units: B region = all k-blocks)
-      }
-      if (tr) P.trace[(size_t)oi * ST_TRACE + 7] = clock64();
-      {
-        const unsigned abar = smem_u32(&acc_full);
-        asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-                     ::"r"(abar) : "memory");
-      }
-      if (tr) P.trace[(size_t)oi * ST_TRACE + 8] = clock64();
-      ++gi;
-    }
-  } else {
-    // =============================== workers: barrier, prologue (B operand), epilogue ===============================
-    const int wt = tid - 64;                  // 0..127
-    const int wq = warp & 3;                  // TMEM lane quadrant this warp may read
-    const int ww = warp - 2;
-    unsigned gi = 0, bar_target = 0;
+  } else if (warp < ST_WORKERS / 32) {
+    // =============================== workers: barrier, prologue (B operand), MMA, epilogue ===============================
+    const int wt = tid;                       // 0..127
+    const int ww = warp;
+    unsigned bar_target = 0;
     unsigned wslot = 0, wph = 0;              // ring position (the workers read K/V pages from the ring; weight tiles are only counted)
     auto ring_advance = [&](unsigned n) { const unsigned adv = wslot + n; wph ^= (adv / (unsigned)NS) & 1u; wslot = adv % (unsigned)NS; };
     // stage descriptors are copied into shared memory ONE STAGE AHEAD (cp.async): read straight from global memory, each first touch of a
-    // descriptor field was an L2/DRAM round trip on the critical path (~1 us per stage, profiles/r02_stream_trace_2.txt)
+    // descriptor field would be an L2/DRAM round trip on the critical path
     constexpr int OPCH = (int)(sizeof(SOp) / 16);
     if (wt < OPCH) cp_async16(s_opbuf[0] + wt * 16, reinterpret_cast<const unsigned char*>(P.ops) + wt * 16, 16);
     cp_async_commit();
@@ -516,9 +530,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
       auto grid_barrier = [&]() {
         if (op.sync_before) {
           if (wt == 0) {
-            // arrival = one fire-and-forget release reduction, then poll the counter.  (Tried, profiles/r02_stream_trace_7.txt: a returning
-            // atomic + release words replicated over 16 lines for the pollers -- 2.6 us from last arrival to last release against 1.5 us for
-            // this form: under the weight stream every dependent L2 round trip costs ~0.7 us, so the form with the fewest of them wins.)
+            // arrival = one fire-and-forget release reduction, then poll the counter: under the weight stream every dependent L2 round
+            // trip is expensive, so the form with the fewest of them wins.
             long long t0 = 0;
             for (unsigned spins = 0; ld_acquire_u32(P.bar_count) < bar_target; ++spins) {
               if ((spins & 255u) == 255u) {
@@ -748,7 +761,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
             }
             if (splice) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             worker_sync();                         // all four warps are done with both pages
-            if (wt == 0) { mbar_arrive(&empty_bar[slotK]); mbar_arrive(&empty_bar[slotV]); }
+            if (lane == 0) { mbar_arrive(&empty_bar[slotK]); mbar_arrive(&empty_bar[slotV]); }
           }
           if (tr && first_seg) P.trace[(size_t)oi * ST_TRACE + 3] = clock64();
           // merge the 4 warps' (m, l, O) and publish this segment's partial
@@ -790,6 +803,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
       if (op.kind != SK_GEMV) break;
       unsigned u0, u1; int KB;
       st_part(op, u0, u1, KB);
+      const unsigned mslot = wslot, mph = wph;          // ring position of this stage's first weight tile
       ring_advance(u1 - u0);
       if (u0 == u1) { grid_barrier(); side_jobs(); break; }
       const int M = op.M, K = op.K, N = op.N, nB = OP_NB(op), half = nB >> 1;
@@ -798,8 +812,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
       const int rt_first = (int)(u0 / (unsigned)KB), kb_first = (int)(u0 - (unsigned)rt_first * (unsigned)KB);
       const int pro = op.pro;
       // ---------------- prologue: ONE batch of L2 loads (row statistics + the first activation chunks), then compute ----------------
-      // (measured, profiles/r02_stream_trace_1.txt: a statistics loop followed by a staging loop costs one L2 round trip per loop
-      //  iteration, 4.4 us per AdaLN stage; every load below is issued before the first value is consumed)
+      // (a statistics loop followed by a staging loop would cost one L2 round trip per loop iteration; every load below is issued before
+      //  the first value is consumed)
       const int total = M * count * 8;                     // 16-byte chunks (8 consecutive k of one activation row) to stage
       const bool norm = (PRO_IS(SP_RMSNORM) || PRO_IS(SP_ADALN));
       // SP_COMBINE scratch behind the B operand: [M][NH][G] merge weights w_p / sum_p w_p l_p | group partial sums | merged[M][count][64]
@@ -1055,7 +1069,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
       if (tr) P.trace[(size_t)oi * ST_TRACE + 10] = clock64();
       if (norm) {
         // sum of squares of every full row: rows in pairs, <= 16 float4 per thread in flight (K <= 4096), further columns looped
-        // (rot: every CTA starts at a different column -- the 148 SMs read the same rows at the same moment, in phase they queue on the
+        // (rot: every CTA starts at a different column -- all SMs read the same rows at the same moment, in phase they queue on the
         //  same L2 lines)
         const float* const sx = op.x; const long long sldx = op.ldx;
         for (int m0 = 0; m0 < M; m0 += 2) {
@@ -1132,91 +1146,22 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy smem writes -> visible to the tensor core
       worker_sync();
-      if (wt == 0) mbar_arrive(&b_ready);
       if (tr) P.trace[(size_t)oi * ST_TRACE + 3] = clock64();
       side_jobs();
-      // ---------------- epilogue ----------------
-      // bias / gamma / gate values do not depend on the MMA: fetch them while it runs (a gate load per segment AFTER the accumulators were
-      // complete cost one L2 round trip per segment and made the CTAs that straddle a row-tile boundary arrive ~0.9 us late at every barrier)
-      const int rt_last = (int)((u1 - 1u) / (unsigned)KB);
-      constexpr int EPRE = 3;                                 // segments whose operands are prefetched (more: loaded in place)
-      float e_bias[EPRE], e_alpha[EPRE][8];
-      // (descriptor fields in registers: read through `op` they are re-loaded from shared memory after every asm statement -- this block
-      //  alone was 200 instructions and 12 % of a worker warp's time in the sampler, profiles/r02_prof_stream2_*)
-      const float* const e_al = op.alpha; const float* const e_bs = op.bias; float* const e_y = op.y;
-      const long long e_lda = op.lda, e_ldy = op.ldy;
-      const bool e_gate = ALPHA_IS(SA_GATE), e_gamma = ALPHA_IS(SA_GAMMA), e_store = op.store != 0;
-#pragma unroll
-      for (int sg = 0; sg < EPRE; ++sg) {
-        const int rt = rt_first + sg;
-        const int n = rt * 128 + wq * 32 + lane;
-        const bool live = rt <= rt_last && n < N;
-        const bool from0 = (sg > 0) || kb_first == 0;
-        e_bias[sg] = (live && from0 && e_bs) ? e_bs[n] : 0.f;
-        const float gam = (live && e_gamma) ? e_al[n] : 1.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) e_alpha[sg][j] = gam;
-        if (e_gate && live) {
-          const float* gp = e_al + n;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (j >= M) break;
-            e_alpha[sg][j] = ldcg1(gp);
-            gp += e_lda;
-          }
-        }
+      {
+        StEpi ep;
+        ep.bias = op.bias; ep.alpha = op.alpha; ep.y = op.y; ep.lda = op.lda; ep.ldy = op.ldy;
+        ep.gate = ALPHA_IS(SA_GATE); ep.gamma = ALPHA_IS(SA_GAMMA); ep.store = op.store != 0;
+        long long* const trs = tr ? P.trace + (size_t)oi * ST_TRACE : nullptr;
+        if (nB == 16) st_mma_epilogue<16>(ring, breg, full_bar, empty_bar, NS, mslot, mph, u0, u1, KB, M, N, ep, P.diag, oi, trs);
+        else if (nB == 32) st_mma_epilogue<32>(ring, breg, full_bar, empty_bar, NS, mslot, mph, u0, u1, KB, M, N, ep, P.diag, oi, trs);
+        else st_mma_epilogue<64>(ring, breg, full_bar, empty_bar, NS, mslot, mph, u0, u1, KB, M, N, ep, P.diag, oi, trs);
       }
-      mbar_wait_wd(&acc_full, gi & 1u, P.diag, 5u, (unsigned)oi, gi);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (tr) P.trace[(size_t)oi * ST_TRACE + 4] = clock64();
-      for (int rt = rt_first; rt <= rt_last; ++rt) {
-        const bool from0 = (rt > rt_first) || kb_first == 0;            // this segment holds k-block 0 of its row tile -> it adds the bias
-        const int n = rt * 128 + wq * 32 + lane;
-        const unsigned tcol = tmem + ((unsigned)(wq * 32) << 16) + (unsigned)((rt - rt_first) * nB);
-        for (int m0 = 0; m0 < half; m0 += 8) {
-          unsigned rh[8], rl[8];
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(rh[0]), "=r"(rh[1]), "=r"(rh[2]), "=r"(rh[3]), "=r"(rh[4]), "=r"(rh[5]), "=r"(rh[6]), "=r"(rh[7]) : "r"(tcol + (unsigned)m0));
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(rl[0]), "=r"(rl[1]), "=r"(rl[2]), "=r"(rl[3]), "=r"(rl[4]), "=r"(rl[5]), "=r"(rl[6]), "=r"(rl[7]) : "r"(tcol + (unsigned)(half + m0)));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (n < N) {
-            const int sg = rt - rt_first;
-            const bool pre = sg < EPRE && m0 == 0;
-            float bias, gam = 1.f;
-            if (sg < EPRE) bias = sg == 0 ? e_bias[0] : (sg == 1 ? e_bias[1] : e_bias[2]);
-            else bias = (from0 && e_bs) ? e_bs[n] : 0.f;
-            if (!pre && e_gamma) gam = e_al[n];
-            float* yp = e_y + (long long)m0 * e_ldy + n;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int m = m0 + j;
-              // uniform early exit: the dead rows of an M = 2 stage were ~50 predicated-off instructions -- 6 % of the sampler's time on
-              // this instruction-fetch-bound path (profiles/r02_ab_epilogue_rows_stats_groups.txt)
-              if (m >= M) break;
-              float val = __uint_as_float(rh[j]) + __uint_as_float(rl[j]) + bias;
-              if (pre) val *= sg == 0 ? e_alpha[0][j] : (sg == 1 ? e_alpha[1][j] : e_alpha[2][j]);
-              else if (e_gate) val *= ldcg1(e_al + (long long)m * e_lda + n);
-              else val *= gam;
-              if (e_store) *yp = val; else red_add_f32(yp, val);
-              yp += e_ldy;
-            }
-          }
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
       if (tr) P.trace[(size_t)oi * ST_TRACE + 5] = clock64();
-      ++gi;
       } while (0);
       cp_async_wait<0>();                      // next stage's descriptor has landed ...
       worker_sync();                           // ... for every worker; also: all workers' global writes of this stage are issued
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
   }
 }
 #undef PRO_IS
@@ -1225,80 +1170,5 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
 #undef ATT_HD
 #undef OP_NB
 
-
-// ---------------------------------------------------------------------------------------------------------------------------------
-// micro-benchmark: issue rate / execution time of tcgen05.mma 128 x nB x 16 from shared memory (operands are whatever the buffer holds)
-//   mode 0: `n` MMAs back to back, one commit at the end; mode 1: commit + mbarrier wait after every 4 MMAs (= one 16 KB weight tile).
-//   `nacc` accumulators are used round-robin (1 = one dependent chain).  out[cta] = SM cycles.
-// ---------------------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int n, int nB, int mode, int nacc, long long* out) {
-  extern __shared__ unsigned char mr_raw[];
-  __shared__ unsigned long long bar;
-  __shared__ unsigned tmem_base_s;
-  const unsigned raw_addr = smem_u32(mr_raw);
-  unsigned char* sm = mr_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  for (int i = tid; i < (8 * ST_TILE + 32768) / 4; i += 128) reinterpret_cast<unsigned*>(sm)[i] = 0x3c003c00u;
-  if (tid == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tmem = tmem_base_s;
-  const unsigned idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(nB >> 3) << 17) | ((unsigned)(128 >> 4) << 24);
-  const unsigned long long db = umma_desc_sw128(smem_u32(sm + 8 * ST_TILE));
-  const unsigned long long da0 = umma_desc_sw128(smem_u32(sm));
-  // modes: 0 one thread (tid 0) issues, single commit; 1 commit + wait per 4; 3 whole warp converged, elect.sync inside the asm; 4 like 0 but
-  //        loop-invariant operands (same A tile, same accumulator): pure issue cost
-  if (mode == 3) {
-    if (warp == 1) {
-      const long long t0 = clock64();
-      for (int i = 0; i < n; ++i) {
-        const unsigned long long da = da0 + (unsigned long long)(((i >> 2) & 7) * (ST_TILE >> 4)) + 2 * (i & 3);
-        const unsigned dcol = tmem + (unsigned)((i % nacc) * nB);
-        const unsigned acc = i >= nacc ? 1u : 0u;
-        asm volatile("{\n\t.reg .pred p, e;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|e, 0xffffffff;\n\t@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(dcol), "l"(da), "l"(db + 2 * (i & 3)), "r"(idesc), "r"(acc) : "memory");
-      }
-      const long long t1 = clock64();
-      if ((tid & 31) == 0) {
-        tc5_commit(&bar);
-        mbar_wait_wd(&bar, 0, nullptr, 9u, 0u, 0u);
-        out[blockIdx.x] = clock64() - t0;
-        out[gridDim.x + blockIdx.x] = t1 - t0;
-      }
-    }
-  } else if (tid == 0) {
-    unsigned phase = 0;
-    const long long t0 = clock64();
-    if (mode == 4) {
-      for (int i = 0; i < n; ++i) tc5_mma(tmem, da0, db, idesc, 1u);
-    } else {
-      for (int i = 0; i < n; ++i) {
-        const unsigned long long da = da0 + (unsigned long long)(((i >> 2) & 7) * (ST_TILE >> 4)) + 2 * (i & 3);
-        tc5_mma(tmem + (unsigned)((i % nacc) * nB), da, db + 2 * (i & 3), idesc, i >= nacc ? 1u : 0u);   // nacc independent accumulators
-        if (mode == 1 && (i & 3) == 3) {
-          tc5_commit(&bar);
-          mbar_wait_wd(&bar, phase, nullptr, 9u, 0u, 0u);
-          phase ^= 1u;
-        }
-      }
-    }
-    const long long t1 = clock64();
-    if (mode != 1) {
-      tc5_commit(&bar);
-      mbar_wait_wd(&bar, 0, nullptr, 9u, 0u, 0u);
-    }
-    out[blockIdx.x] = clock64() - t0;
-    out[gridDim.x + blockIdx.x] = t1 - t0;       // issue loop only
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-}
 
 }  // namespace vv

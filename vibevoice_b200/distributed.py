@@ -1,7 +1,7 @@
 """Multi-GPU plumbing (SURVEY 8e): prompts shard by batch across ranks -- one process per GPU, weights replicated, no
 collective inside the generation loop -- and the finished waveforms are gathered to rank 0 with one exchange of lengths
-(`all_gather`) and one `gather` of zero-padded samples.  Works on any `torch.distributed` backend (NCCL over NVLink on the
-GPU box, gloo in the CPU tests)."""
+(`all_gather`) and one `gather` of zero-padded samples.  Works on any `torch.distributed` backend (NCCL over NVLink on a
+multi-GPU machine, gloo in the CPU tests)."""
 from __future__ import annotations
 
 from typing import List, Optional, Sequence

@@ -1,6 +1,6 @@
 """Device engine: owns one `vv_ctx` (C ABI, `include/vibevoice_b200.h`), the persistent I/O buffers the
 captured CUDA graphs are bound to, and the stream they run on.  Pure plumbing -- all arithmetic is in
-`csrc/` (hand-written sm_100a kernels).  PyTorch is used for device memory and streams only.
+`csrc/` (hand-written sm_90a kernels).  PyTorch is used for device memory and streams only.
 """
 from __future__ import annotations
 
@@ -56,7 +56,7 @@ class Engine:
 
     def __init__(self, config: VibeVoiceConfig, valid_ids, max_batch: int = 1, device: int = 0, max_diffusion_steps: int = 64):
         if not torch.cuda.is_available():
-            raise N.VVError("vibevoice_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise N.VVError("vibevoice_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = N.load_library()
         if self.lib.vv_abi_version() != 1:
             raise N.VVError("ABI mismatch")

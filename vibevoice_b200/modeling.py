@@ -1,5 +1,5 @@
 """`VibeVoiceForConditionalGenerationInference` -- the reference's public generation surface
-(`vibevoice/modular/modeling_vibevoice_inference.py:68-717`) on top of the B200 engine.
+(`vibevoice/modular/modeling_vibevoice_inference.py:68-717`) on top of the H100 engine.
 
 Same constructor / `from_pretrained` / `set_ddpm_inference_steps` / `generate(**kwargs)` contract and the
 same `VibeVoiceGenerationOutput`, so `demo/inference_from_file.py:280-431` runs against this class.  The loop

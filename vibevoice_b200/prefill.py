@@ -108,6 +108,12 @@ class TorchVoicePrompt:
     @torch.no_grad()
     def encode_mean(self, wavs: torch.Tensor) -> torch.Tensor:
         """wavs [n, T] -> latent means [n, ceil(T/3200), vae_dim]"""
+        # cuDNN may run fp32 convolutions in TF32 unless told otherwise; the encoder is meant to be fp32
+        cd = torch.backends.cudnn
+        with cd.flags(enabled=cd.enabled, benchmark=cd.benchmark, deterministic=cd.deterministic, allow_tf32=False):
+            return self._encode_mean(wavs)
+
+    def _encode_mean(self, wavs: torch.Tensor) -> torch.Tensor:
         tc, p, w = self.tc, self.ENC, self.w
         x = wavs.to(self.device, torch.float32)[:, None, :]
         depths, ratios = tc.encoder_depth_list, list(reversed(tc.encoder_ratios))

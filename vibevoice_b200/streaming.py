@@ -15,10 +15,10 @@ What differs from the multi-speaker loop (`modeling.py`), and how it maps onto t
 Batch size 1, like the reference (`:511`).
 
 STATUS: host logic held to fixtures from the reference's own streaming generate() on the CPU through the engine stand-in
-(`tests/test_host_logic.py::test_streaming_product_host_logic_against_reference_fixture`); CUDA path vs the pinned oracle on B200
+(`tests/test_host_logic.py::test_streaming_product_host_logic_against_reference_fixture`); CUDA path vs the pinned oracle on the GPU
 (`tests/test_gpu_parity.py::test_streaming_variant_vs_oracle`, sequences exact, audio 4e-6) and at the shipped 0.5B shapes (24 layers split
 4 / 20, H = 896, 14 query / 2 KV heads, head_dim 64: `tests/test_gpu_scale.py::test_streaming_variant_real_05b_shapes_vs_oracle`); first-audio
-latency harness: `python bench.py --model streaming-0.5b` (p50 6.2 ms at an 8 K cached prompt, profiles/r02_streaming_05b_first_audio_latency_final.json).
+latency harness: `python bench.py --model streaming-0.5b` (8 K cached prompt).
 """
 from __future__ import annotations
 
