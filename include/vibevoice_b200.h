@@ -167,6 +167,14 @@ int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_ou
  * prologue: 0 none, 1 RMSNorm(pro_w, eps), 3 SwiGLU pairs (x is [M][2K]), 4 GELU, 6 SiLU; alpha_kind: 0 one, 2 gamma[n]. Synchronises. */
 int vv_debug_stream_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, float* y, int M, int N, int K, int prologue,
                          const float* pro_w, float eps, int alpha_kind, const float* alpha, int accumulate, void* stream);
+/* the same linear with every stage feature exposed: y[m][n] = (store ? 0 : y[m][n]) + alpha * (W pro(x[m]) + bias[n]), rows of x / y
+ * ldx / ldy floats apart (SwiGLU: x rows hold 2K interleaved gate / up sums).  prologue 2 = AdaLN: RMSNorm(pro_w or 1, eps) * (1 + scale) +
+ * shift with scale / shift rows pro_ld floats apart; alpha_kind 1 = gate alpha[m][n] (row stride lda), 2 = gamma alpha[n].  store needs
+ * K <= 64.  operand_cap > 0 caps the activation-operand bytes of the stage, so that smaller shapes run through the K split as well.
+ * Synchronises; returns the number of stages the linear ran as (> 1: split along K). */
+int vv_debug_stream_gemv2(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, int64_t ldx, float* y, int64_t ldy, int M, int N,
+                          int K, int prologue, const float* pro_w, float eps, const float* pro_shift, const float* pro_scale, int64_t pro_ld,
+                          int alpha_kind, const float* alpha, int64_t lda, int store, int64_t operand_cap, void* stream);
 int vv_stream_trace_read2(vv_ctx* ctx, long long* out /*[max_ops][sm_count][2]*/, int max_ops);  /* every CTA's barrier arrival / release (globaltimer ns); returns sm_count */
 int vv_stream_trace_read(vv_ctx* ctx, long long* out /*[max_ops][12]*/, int* out_meta /*[max_ops][4]*/, int max_ops, const char* program_prefix);
                                                    /* VV_STREAM_TRACE=<cta>: per-stage clock stamps of one CTA of the last traced launch */

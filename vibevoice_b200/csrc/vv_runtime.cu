@@ -21,6 +21,7 @@
 #include <map>
 #include <set>
 #include <string>
+#include <tuple>
 #include <vector>
 
 using namespace vv;
@@ -134,7 +135,10 @@ struct vv_ctx {
   std::map<std::string, GraphEntry> graphs;
   GridBar* gridbar = nullptr;
   // weight-stream programs (vv_stream.cuh)
-  struct StreamProg { SOp* ops = nullptr; int n_ops = 0; CUtensorMap* tmaps = nullptr; int n_stages = 0; int b_bytes = 0; int smem = 0; int gemv_ops = 0; int variant = 0; };
+  struct StreamProg {
+    SOp* ops = nullptr; int n_ops = 0; CUtensorMap* tmaps = nullptr; int n_stages = 0; int b_bytes = 0; int smem = 0; int gemv_ops = 0; int variant = 0;
+    std::vector<int> op_first;           // stage i as built -> its first stage in `ops` (a K-split stage becomes several)
+  };
   std::map<std::string, StreamProg> sprogs;
   unsigned* st_bar = nullptr;            // grid-barrier counter of the stream kernel
   unsigned* st_diag_host = nullptr; unsigned* st_diag_dev = nullptr;   // host-mapped watchdog record
@@ -145,7 +149,8 @@ struct vv_ctx {
                                          // through the weight-stream kernel; 0 -> kernel-per-stage everywhere
   float* s_rope = nullptr;                        // [2B][64][2] cos / sin of the current positions
   float *s_pacc2 = nullptr, *s_pml2 = nullptr;   // attention partials of the stream path: [2B][kv_heads][SMs][8][128] / [..][8][2]
-  std::map<const bf16*, bf16*> tiled; size_t tiled_bytes = 0;   // tile-major copies of the weights the stream kernel reads
+  std::map<std::tuple<const bf16*, int, int>, bf16*> tiled; size_t tiled_bytes = 0;   // tile-major copies of the weights the stream kernel reads,
+                                                                                         // per (weight, first column, columns)
   long long* st_trace2 = nullptr;
   long long* st_trace = nullptr; int st_trace_ops = 0; int st_trace_cta = 0; int st_trace_last_ops = 0;   // VV_STREAM_TRACE=<cta>: per-stage clock stamps of one CTA
   float* cfg_dev = nullptr; float cfg_last = NAN;   // CFG scale lives in device memory so captured graphs do not depend on its value
@@ -328,22 +333,25 @@ static int make_weight_tmap(const bf16* T, long long n_tiles, CUtensorMap* out) 
   if (r != CUDA_SUCCESS) return fail(VV_ERR_CUDA, "cuTensorMapEncodeTiled([%d tiles x %d]) failed with %d", N, K, (int)r);
   return 0;
 }
-// tile-major copy of W [N][K] (cached per weight pointer; `fresh` = never cache: the caller's buffer may be re-used with other contents)
-static int tiled_weight(vv_ctx* c, const bf16* W, int N, int K, bool fresh, bf16** out, long long* n_tiles) {
-  if (K % 8 || ((uintptr_t)W & 15)) return fail(VV_ERR_INVALID, "stream: weight [%d x %d] must have K %% 8 == 0 and a 16-byte aligned base", N, K);
+// tile-major copy of columns [k0, k0 + K) of W [N][ldw] (cached per weight pointer and column range; `fresh` = never cache: the caller's
+// buffer may be re-used with other contents)
+static int tiled_weight(vv_ctx* c, const bf16* W, long long ldw, int N, int K, int k0, bool fresh, bf16** out, long long* n_tiles) {
+  if (K % 8 || k0 % 8 || ldw % 8 || ((uintptr_t)W & 15))
+    return fail(VV_ERR_INVALID, "stream: weight [%d x %d] must have K %% 8 == 0 and a 16-byte aligned base", N, K);
   const long long KB = (K + 63) / 64, R = (N + 127) / 128;
   *n_tiles = R * KB;
+  const auto key = std::make_tuple(W, k0, K);
   if (!fresh) {
-    auto it = c->tiled.find(W);
+    auto it = c->tiled.find(key);
     if (it != c->tiled.end()) { *out = it->second; return 0; }
   }
   bf16* T = nullptr;
   RET(dmalloc(c, &T, (size_t)(*n_tiles) * 8192, false));
   const long long n_chunks = *n_tiles * 1024;
-  tile_pack_kernel<<<(unsigned)std::min<long long>((n_chunks + 255) / 256, (long long)c->sm_count * 32), 256>>>(W, T, N, K, (int)KB, n_chunks);
+  tile_pack_kernel<<<(unsigned)std::min<long long>((n_chunks + 255) / 256, (long long)c->sm_count * 32), 256>>>(W, T, N, K, (int)KB, ldw, k0, n_chunks);
   CKL();
   CK(cudaDeviceSynchronize());
-  if (!fresh) c->tiled[W] = T;
+  if (!fresh) c->tiled[key] = T;
   c->tiled_bytes += (size_t)(*n_tiles) * 16384;
   *out = T;
   return 0;
@@ -353,18 +361,20 @@ struct StreamBuilder {
   vv_ctx* c;
   std::vector<SOp> ops;
   std::vector<CUtensorMap> tmaps;
-  std::vector<int> tmap_of;        // op -> tensor map index (or -1)
+  std::vector<const bf16*> wsrc;   // op -> weight [N][K] of a linear stage (else null); sliced, packed and mapped by finish_stream
   explicit StreamBuilder(vv_ctx* c_) : c(c_) {}
   SOp& push(int kind, bool sync) {
     SOp o;
     memset(&o, 0, sizeof o);
     o.kind = kind; o.sync_before = sync ? 1 : 0; o.nB = 16;
-    ops.push_back(o); tmap_of.push_back(-1);
+    ops.push_back(o); wsrc.push_back(nullptr);
     return ops.back();
   }
   // y[m][n] (+)= alpha * (W x'[m] + bias); x' = pro(x)
   bool fresh_weights = false;
   std::vector<bf16*> owned;         // tile-major copies made with fresh_weights (freed by the caller)
+  long long operand_cap = 0;        // > 0: bytes a linear stage's operand region may take before it is split along K (default: what leaves
+                                    // ST_MIN_RING ring slots)
   int kv_tmap = -1;                 // index of the K-pool tensor map (V-pool map follows) for SK_ATTN stages
   std::vector<int> needs_kv;        // ops whose att.tmap_k / tmap_v must be patched
   int use_kv_pool() {
@@ -410,16 +420,12 @@ struct StreamBuilder {
   }
   int gemv(const bf16* W, const float* bias, const float* x, long long ldx, float* y, long long ldy, int M, int N, int K, bool sync, SOp** out) {
     if (M < 1 || M > 32) return fail(VV_ERR_INVALID, "stream gemv: M=%d outside [1,32]", M);
-    CUtensorMap tm;
-    bf16* T; long long n_tiles;
-    RET(tiled_weight(c, W, N, K, fresh_weights, &T, &n_tiles));
-    if (fresh_weights) owned.push_back(T);
-    RET(make_weight_tmap(T, n_tiles, &tm));
+    if (N < 1 || K < 8 || K % 8 || ((uintptr_t)W & 15))
+      return fail(VV_ERR_INVALID, "stream: weight [%d x %d] must have K %% 8 == 0 and a 16-byte aligned base", N, K);
     SOp& o = push(SK_GEMV, sync);
-    o.M = M; o.N = N; o.K = K; o.nB = M <= 8 ? 16 : (M <= 16 ? 32 : 64);
+    o.M = M; o.N = N; o.K = K; o.krow = K; o.nB = M <= 8 ? 16 : (M <= 16 ? 32 : 64);
     o.x = x; o.ldx = ldx; o.y = y; o.ldy = ldy; o.bias = bias; o.pro = SP_NONE; o.alpha_kind = SA_ONE;
-    tmaps.push_back(tm);
-    tmap_of.back() = (int)tmaps.size() - 1;
+    wsrc.back() = W;
     *out = &ops.back();
     return 0;
   }
@@ -454,31 +460,83 @@ static const struct { unsigned feat; StreamFn fn; StreamFn fn_trace; const char*
 #undef SVAR
 constexpr int N_STREAM_VARIANTS = 8;
 
+constexpr int ST_MIN_RING = 3;    // ring slots a program must keep: a linear stage whose operand region leaves fewer is split along K
+
+// Bytes of the operand region a linear stage needs when it reduces over KBs k-blocks: the B operand of every k-block a CTA touches (+ the
+// attention-merge scratch of SP_COMBINE: merge weights, group partial sums, merged rows).  *heads = distinct heads per CTA (SP_COMBINE).
+static long long stage_operand_bytes(const vv_ctx* c, const SOp& o, long long KBs, long long* heads) {
+  const int G = c->sm_count;
+  const long long R = (o.N + 127) / 128, per = (R * KBs + G - 1) / G, count = std::min(per, KBs);
+  long long bytes = count * o.nB * 128;
+  *heads = 0;
+  if (o.pro == SP_COMBINE) {
+    const long long kbh = c->d.head_dim / 64, nh = (count + kbh - 2) / kbh + 2;
+    *heads = nh;
+    bytes = ((bytes + 1023) & ~1023ll) + o.M * nh * G * 4 + 16 + std::max<long long>(2048, o.M * count * 256) + o.M * count * 256;
+  }
+  return bytes;
+}
+
+// K split: y += alpha * W pro(x) is a sum over k-blocks and the epilogue is an atomic sum, so a stage whose operand region is too large
+// for the ring runs as consecutive slices over k-block ranges (SP_COMBINE: whole heads).  The first slice keeps the grid barrier, bias,
+// zero-fill jobs and RoPE rows; the others follow without a barrier.  Every slice has its own tile-major weight copy and tensor map.
+// first[i] = index of the first stage that stage i of the builder became (first[n] = stage count).
+static int split_and_map(StreamBuilder& b, long long cap, std::vector<int>* tmap_of, std::vector<int>* first_out) {
+  vv_ctx* c = b.c;
+  std::vector<SOp> ops;
+  std::vector<int>& first = *first_out;
+  first.assign(b.ops.size() + 1, 0);
+  tmap_of->clear();
+  for (size_t i = 0; i < b.ops.size(); ++i) {
+    first[i] = (int)ops.size();
+    const SOp& o = b.ops[i];
+    if (o.kind != SK_GEMV) { ops.push_back(o); tmap_of->push_back(-1); continue; }
+    const long long KB = (o.K + 63) / 64;
+    const long long gran = o.pro == SP_COMBINE ? c->d.head_dim / 64 : 1;
+    const bool can_split = o.pro != SP_DPM && o.pro != SP_WINDOW && !o.store;
+    auto fits = [&](long long kbs) {
+      long long nh;
+      const long long bytes = stage_operand_bytes(c, o, kbs, &nh);
+      return bytes <= cap && o.M * nh <= 128;
+    };
+    long long kbs = KB;
+    if (can_split && !fits(KB))
+      for (long long s = 2; s <= KB; ++s) {
+        kbs = ((KB + s - 1) / s + gran - 1) / gran * gran;
+        if (fits(kbs) || kbs <= gran) break;
+      }
+    for (long long kb0 = 0; kb0 < KB; kb0 += kbs) {
+      SOp so = o;
+      so.k0 = (int)(kb0 * 64);
+      so.K = (int)std::min<long long>(kbs * 64, o.K - so.k0);
+      if (kb0 > 0) {
+        so.sync_before = 0; so.bias = nullptr; so.rope_rows = 0;
+        so.init_dst = nullptr; so.init_n = 0; so.init2_dst = nullptr; so.init2_n = 0;
+      }
+      bf16* T; long long n_tiles;
+      RET(tiled_weight(c, b.wsrc[i], o.K, o.N, so.K, so.k0, b.fresh_weights, &T, &n_tiles));
+      if (b.fresh_weights) b.owned.push_back(T);
+      CUtensorMap tm;
+      RET(make_weight_tmap(T, n_tiles, &tm));
+      b.tmaps.push_back(tm);
+      ops.push_back(so); tmap_of->push_back((int)b.tmaps.size() - 1);
+    }
+  }
+  first[b.ops.size()] = (int)ops.size();
+  std::vector<int> needs_kv;
+  for (int i : b.needs_kv)
+    for (int j = first[i]; j < first[i + 1]; ++j) needs_kv.push_back(j);
+  if (getenv("VV_VERBOSE") && ops.size() != b.ops.size())
+    fprintf(stderr, "[vv] stream program: %zu stages after the K split of %zu\n", ops.size(), b.ops.size());
+  b.ops.swap(ops);
+  b.needs_kv.swap(needs_kv);
+  b.wsrc.assign(b.ops.size(), nullptr);
+  return 0;
+}
+
 static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
   vv_ctx* c = b.c;
   const int G = c->sm_count;
-  int b_bytes = 2048;
-  for (const SOp& o : b.ops) {
-    if (o.kind == SK_MIX && (o.cod.T_out > 8 || o.K % 4 || o.K > 4096)) return fail(VV_ERR_INVALID, "stream: mixer stage handles T <= 8, C <= 4096");
-    if (o.kind == SK_ATTN) b_bytes = std::max(b_bytes, 32768);        // Q tile, new K/V row and the warp-merge buffers live in the operand region
-    if (o.kind != SK_GEMV) continue;
-    const long long KB = (o.K + 63) / 64, R = (o.N + 127) / 128, U = R * KB;
-    const long long per = (U + G - 1) / G;
-    const long long count = std::min(per, KB);
-    b_bytes = std::max<long long>(b_bytes, count * o.nB * 128);
-    const long long segs = (per + KB - 1) / KB + 1;
-    if (segs > ST_MAXSEG) return fail(VV_ERR_INVALID, "stream: stage [%d x %d] needs %lld accumulators per CTA", o.N, o.K, segs);
-    if (o.store && KB != 1) return fail(VV_ERR_INVALID, "stream: store epilogue needs K <= 64");
-    if (o.pro == SP_WINDOW && (o.cod.cin % 8)) return fail(VV_ERR_INVALID, "stream: window prologue needs a channel count that is a multiple of 8");
-    if (o.pro == SP_COMBINE) {
-      const long long nh = count / 2 + 2;
-      if ((long long)o.M * nh > 128 || KB != (c->d.head_dim / 64) * c->d.num_q_heads)
-        return fail(VV_ERR_INVALID, "stream: attention-merge prologue does not fit (M=%d, %lld k-blocks per CTA)", o.M, count);
-      b_bytes = std::max<long long>(b_bytes, ((count * o.nB * 128 + 1023) & ~1023ll) + o.M * nh * G * 4 + 16 + std::max<long long>(2048, o.M * count * 256) +
-                                                 o.M * count * 256);
-    }
-    if (U * (G + 1) >= (1ll << 32)) return fail(VV_ERR_INVALID, "stream: stage [%d x %d] has too many tiles for 32-bit scheduling", o.N, o.K);
-  }
   unsigned feat = 0;
   bool hd128 = true, nb16 = true;
   for (const SOp& o : b.ops) {
@@ -495,6 +553,29 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
   cudaFuncAttributes fa;
   CK(cudaFuncGetAttributes(&fa, STREAM_VARIANTS[pr->variant].fn));
   const int max_dyn = 232448 - (int)fa.sharedSizeBytes - 256;
+  std::vector<int> tmap_of;
+  RET(split_and_map(b, b.operand_cap > 0 ? b.operand_cap : (long long)max_dyn - 1024 - (long long)ST_MIN_RING * ST_TILE, &tmap_of, &pr->op_first));
+  int b_bytes = 2048;
+  for (const SOp& o : b.ops) {
+    if (o.kind == SK_MIX && (o.cod.T_out > 8 || o.K % 4 || o.K > 4096)) return fail(VV_ERR_INVALID, "stream: mixer stage handles T <= 8, C <= 4096");
+    if (o.kind == SK_ATTN) b_bytes = std::max(b_bytes, 32768);        // Q tile, new K/V row and the warp-merge buffers live in the operand region
+    if (o.kind != SK_GEMV) continue;
+    const long long KB = (o.K + 63) / 64, R = (o.N + 127) / 128, U = R * KB;
+    const long long per = (U + G - 1) / G;
+    long long nh;
+    b_bytes = std::max<long long>(b_bytes, stage_operand_bytes(c, o, KB, &nh));
+    const long long segs = (per + KB - 1) / KB + 1;
+    if (segs > ST_MAXSEG) return fail(VV_ERR_INVALID, "stream: stage [%d x %d] needs %lld accumulators per CTA", o.N, o.K, segs);
+    if (o.store && KB != 1) return fail(VV_ERR_INVALID, "stream: store epilogue needs K <= 64");
+    if (o.pro == SP_WINDOW && (o.cod.cin % 8)) return fail(VV_ERR_INVALID, "stream: window prologue needs a channel count that is a multiple of 8");
+    if (o.pro == SP_COMBINE) {
+      const int hd = c->d.head_dim;
+      if ((long long)o.M * nh > 128 || o.k0 % hd || o.K % hd || o.k0 + o.K > hd * c->d.num_q_heads)
+        return fail(VV_ERR_INVALID, "stream: attention-merge prologue does not fit (M=%d, heads %d..%d, %lld per CTA)", o.M, o.k0 / hd,
+                    (o.k0 + o.K) / hd, nh);
+    }
+    if (U * (G + 1) >= (1ll << 32)) return fail(VV_ERR_INVALID, "stream: stage [%d x %d] has too many tiles for 32-bit scheduling", o.N, o.K);
+  }
   int ns = (max_dyn - 1024 - b_bytes) / ST_TILE;
   ns = std::min(ns, ST_MAX_STAGES);
   if (getenv("VV_STREAM_STAGES")) ns = std::min(ns, atoi(getenv("VV_STREAM_STAGES")));
@@ -508,7 +589,7 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
     b.ops[i].att.tmap_v = (unsigned long long)(uintptr_t)(pr->tmaps + b.kv_tmap + 1);
   }
   for (size_t i = 0; i < b.ops.size(); ++i) {
-    if (b.tmap_of[i] >= 0) b.ops[i].tmap = (unsigned long long)(uintptr_t)(pr->tmaps + b.tmap_of[i]);
+    if (tmap_of[i] >= 0) b.ops[i].tmap = (unsigned long long)(uintptr_t)(pr->tmaps + tmap_of[i]);
     pr->gemv_ops += b.ops[i].kind == SK_GEMV;
   }
   if (!b.tmaps.empty()) CK(cudaMemcpy(pr->tmaps, b.tmaps.data(), b.tmaps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
@@ -518,9 +599,15 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
   return 0;
 }
 
+// stages [op_begin, op_begin + op_count) of the program as built (-1: to the end), i.e. with all the slices of K-split stages
 static int launch_stream(const L& l, const vv_ctx::StreamProg& pr, int op_begin = 0, int op_count = -1) {
   vv_ctx* c = l.c;
-  if (op_count < 0) op_count = pr.n_ops - op_begin;
+  const int n_built = (int)pr.op_first.size() - 1;
+  if (op_count < 0) op_count = n_built - op_begin;
+  if (op_begin < 0 || op_begin + op_count > n_built) return fail(VV_ERR_INVALID, "stream: stages [%d, +%d) outside the program", op_begin, op_count);
+  const int op_end = pr.op_first[op_begin + op_count];
+  op_begin = pr.op_first[op_begin];
+  op_count = op_end - op_begin;
   CK(cudaMemsetAsync(c->st_bar, 0, sizeof(unsigned), l.s));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
@@ -2118,6 +2205,24 @@ extern "C" int vv_debug_gemv(vv_ctx* c, const void* w, const float* bias, const 
   return linear(l, p);
 }
 
+// builds, runs and frees a one-off stream program (tests); returns the number of stages it ran (after the K split)
+static int run_debug_stream(vv_ctx* c, StreamBuilder& b, void* stream) {
+  vv_ctx::StreamProg pr;
+  int rc = finish_stream(b, &pr);
+  if (rc == 0) {
+    L l{c, (cudaStream_t)stream};
+    rc = launch_stream(l, pr);
+    if (rc == 0 && cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess) rc = fail(VV_ERR_CUDA, "stream kernel: %s", cudaGetErrorString(cudaGetLastError()));
+  }
+  if (pr.ops) dfree(c, &pr.ops);
+  if (pr.tmaps) dfree(c, &pr.tmaps);
+  for (bf16* t : b.owned) dfree(c, &t);
+  if (rc < 0) return rc;
+  if (c->st_diag_host[0]) return fail(VV_ERR_CUDA, "stream kernel watchdog: code %u cta %u thread %u a %u b %u c %u", c->st_diag_host[0], c->st_diag_host[1],
+                                      c->st_diag_host[2], c->st_diag_host[3], c->st_diag_host[4], c->st_diag_host[5]);
+  return pr.n_ops;
+}
+
 // one linear through the weight-stream kernel (tests): y = [y +] alpha * (W pro(x) + bias); pro = SPro, alpha_kind = SAlpha
 extern "C" int vv_debug_stream_gemv(vv_ctx* c, const void* w, const float* bias, const float* x, float* y, int M, int N, int K, int pro,
                                     const float* pro_w, float eps, int alpha_kind, const float* alpha, int accumulate, void* stream) {
@@ -2129,16 +2234,32 @@ extern "C" int vv_debug_stream_gemv(vv_ctx* c, const void* w, const float* bias,
   SOp* o;
   RET(b.gemv((const bf16*)w, bias, x, pro == SP_SWIGLU ? 2LL * K : (long long)K, y, N, M, N, K, !accumulate, &o));
   o->pro = pro; o->pro_w = pro_w; o->pro_eps = eps; o->alpha_kind = alpha_kind; o->alpha = alpha; o->lda = N;
-  vv_ctx::StreamProg pr;
-  RET(finish_stream(b, &pr));
-  L l{c, (cudaStream_t)stream};
-  RET(launch_stream(l, pr));
-  CK(cudaStreamSynchronize((cudaStream_t)stream));
-  dfree(c, &pr.ops); dfree(c, &pr.tmaps);
-  for (bf16* t : b.owned) dfree(c, &t);
-  if (c->st_diag_host[0]) return fail(VV_ERR_CUDA, "stream kernel watchdog: code %u cta %u thread %u a %u b %u c %u", c->st_diag_host[0], c->st_diag_host[1],
-                                      c->st_diag_host[2], c->st_diag_host[3], c->st_diag_host[4], c->st_diag_host[5]);
-  return 0;
+  const int rc = run_debug_stream(c, b, stream);
+  return rc < 0 ? rc : 0;
+}
+
+// vv_debug_stream_gemv with the strides, AdaLN operands, store epilogue and K split exposed (see the header)
+extern "C" int vv_debug_stream_gemv2(vv_ctx* c, const void* w, const float* bias, const float* x, int64_t ldx, float* y, int64_t ldy, int M, int N, int K,
+                                     int pro, const float* pro_w, float eps, const float* pro_shift, const float* pro_scale, int64_t pro_ld,
+                                     int alpha_kind, const float* alpha, int64_t lda, int store, int64_t operand_cap, void* stream) {
+  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  if (pro != SP_NONE && pro != SP_RMSNORM && pro != SP_ADALN && pro != SP_SWIGLU && pro != SP_GELU && pro != SP_SILU)
+    return fail(VV_ERR_INVALID, "vv_debug_stream_gemv2: prologue %d not supported", pro);
+  if (alpha_kind != SA_ONE && alpha_kind != SA_GATE && alpha_kind != SA_GAMMA) return fail(VV_ERR_INVALID, "vv_debug_stream_gemv2: alpha_kind %d", alpha_kind);
+  if ((pro == SP_ADALN && (!pro_shift || !pro_scale)) || (alpha_kind != SA_ONE && !alpha))
+    return fail(VV_ERR_INVALID, "vv_debug_stream_gemv2: missing AdaLN / alpha operand");
+  if (ldx < (pro == SP_SWIGLU ? 2LL * K : (long long)K) || ldy < N || (alpha_kind == SA_GATE && lda < N) || (pro == SP_ADALN && pro_ld < K) ||
+      ((uintptr_t)x & 15) || ldx % 4 || (pro == SP_ADALN && (pro_ld % 4 || ((uintptr_t)pro_shift & 15) || ((uintptr_t)pro_scale & 15))))
+    return fail(VV_ERR_INVALID, "vv_debug_stream_gemv2: strides must cover the row and keep rows 16-byte aligned");
+  CK(cudaSetDevice(c->device));
+  StreamBuilder b(c);
+  b.fresh_weights = true;
+  b.operand_cap = operand_cap;
+  SOp* o;
+  RET(b.gemv((const bf16*)w, bias, x, ldx, y, ldy, M, N, K, false, &o));
+  o->pro = pro; o->pro_w = pro_w; o->pro_eps = eps; o->pro_shift = pro_shift; o->pro_scale = pro_scale; o->pro_ld = pro_ld;
+  o->alpha_kind = alpha_kind; o->alpha = alpha; o->lda = lda; o->store = store ? 1 : 0;
+  return run_debug_stream(c, b, stream);
 }
 // clock stamps of the last traced stream launch (VV_STREAM_TRACE=<cta>): out [n_ops][12] int64; returns the number of stages, 0 if tracing is off.
 // Stage kinds / shapes are appended per stage in out_meta [n_ops][4] = {kind, N, K, prologue}.

@@ -153,6 +153,8 @@ struct alignas(16) SOp {
   int sync_before;          // wait until every CTA has finished the previous stage (grid barrier) before touching activations
   int M, N, K;              // activation rows, weight rows (outputs), reduction length (K % 8 == 0)
   int nB;                   // MMA N: 16, 32 or 64 (rows [0,nB/2) = hi, [nB/2,nB) = lo)
+  int k0, krow;             // K-split slice: this stage reduces over columns [k0, k0 + K) of rows krow long (x, pro_w, pro_scale / shift,
+                            // SP_COMBINE heads are addressed at k0 + k; RMSNorm / AdaLN statistics always cover the whole krow-long row)
   unsigned long long tmap;  // device address of the CUtensorMap of the TILE-MAJOR copy of W: [R*KB tiles][128 rows][64 k] bf16, zero padded
                             // (seen as a 2-D tensor [R*KB*128][64]; box 64 x 128 = one contiguous 16 KB tile, SWIZZLE_128B)
   int pro;
@@ -188,14 +190,15 @@ constexpr int ST_TRACE = 12;   // 0 op start, 1 barrier passed, 2 row stats done
 
 // W [N][K] row-major -> tile-major [R][KB][128][64], zero padded.  TMA boxes cut out of the row-major matrix (128 rows x 128 B, kilobytes
 // apart) make every row its own DRAM burst, so the kernel reads tiles that are contiguous in HBM instead; units of a stage are consecutive tiles, i.e. every CTA reads ONE contiguous byte range per stage.
-__global__ void tile_pack_kernel(const bf16* __restrict__ W, bf16* __restrict__ T, int N, int K, int KB, long long n_chunks) {
+// A K-split slice packs columns [k0, k0 + K) of a W whose rows are ldw long.
+__global__ void tile_pack_kernel(const bf16* __restrict__ W, bf16* __restrict__ T, int N, int K, int KB, long long ldw, int k0, long long n_chunks) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_chunks; i += (long long)gridDim.x * blockDim.x) {
     const int ch = (int)(i & 7), r = (int)((i >> 3) & 127);
     const long long tile = i >> 10;
     const int kb = (int)(tile % KB), rt = (int)(tile / KB);
     const int n = rt * 128 + r, k = kb * 64 + ch * 8;
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (n < N && k < K) v = *reinterpret_cast<const uint4*>(W + (size_t)n * K + k);       // K % 8 == 0: a chunk never straddles K
+    if (n < N && k < K) v = *reinterpret_cast<const uint4*>(W + (size_t)n * ldw + k0 + k);   // K % 8 == 0: a chunk never straddles K
     *reinterpret_cast<uint4*>(T + i * 8) = v;
   }
 }
@@ -836,18 +839,19 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
         r.fresh = false;
         r.xr = op.x; r.pw = nullptr; r.psc = nullptr; r.psh = nullptr;
         if (!r.live) return r;
+        const int ka = r.k + op.k0;                          // column of the full row (r.k: column of this stage's slice)
         if (PRO_IS(SP_WINDOW)) {
           const SCodec& w = op.cod;
-          const int b = r.m / w.T_out, t = r.m - b * w.T_out, j = r.k / w.cin, ci = r.k - j * w.cin, rr = t * w.stride + j;
+          const int b = r.m / w.T_out, t = r.m - b * w.T_out, j = ka / w.cin, ci = ka - j * w.cin, rr = t * w.stride + j;
           r.fresh = rr >= w.ctx;
           r.xr = rr < w.ctx ? w.hist + ((size_t)b * w.ctx + rr) * w.cin + ci : w.src + ((size_t)b * w.T_in + (rr - w.ctx)) * w.cin + ci;
         } else if (PRO_IS(SP_SWIGLU)) {
-          r.xr = op.x + (long long)r.m * op.ldx + 2 * r.k;
+          r.xr = op.x + (long long)r.m * op.ldx + 2 * ka;
         } else {
-          r.xr = op.x + (long long)r.m * op.ldx + r.k;
-          if (norm && op.pro_w) r.pw = op.pro_w + r.k;
+          r.xr = op.x + (long long)r.m * op.ldx + ka;
+          if (norm && op.pro_w) r.pw = op.pro_w + ka;
           if (PRO_IS(SP_ADALN)) {
-            const long long o = (long long)r.m * op.pro_ld + r.k;
+            const long long o = (long long)r.m * op.pro_ld + ka;
             r.psc = op.pro_scale + o; r.psh = op.pro_shift + o;
           }
         }
@@ -934,7 +938,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
         *reinterpret_cast<uint4*>(blk + (rl >> 3) * 1024 + (rl & 7) * 128 + ((ch ^ (rl & 7)) << 4)) = lv;
       };
       ChunkRef r0 = chunk_ref(wt), r1 = chunk_ref(wt + ST_WORKERS);
-      const int K4 = K >> 2;
+      const int K4 = op.krow >> 2;                          // row statistics: the whole row, also in a K-split slice
       int rot = (int)((blockIdx.x * 67u) % (unsigned)(K4 > 0 ? K4 : 1));     // statistics loads: every CTA starts at a different column
       // materialise the descriptor-only values HERE, ahead of the barrier (the compiler would otherwise sink them to their first use)
       asm volatile("" : "+l"(r0.xr), "+r"(r0.m), "+r"(r0.k), "+r"(r0.jloc), "+l"(r1.xr), "+r"(r1.m), "+r"(r1.k), "+r"(r1.jloc), "+r"(rot));
@@ -943,11 +947,13 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
       const bool cmb = PRO_IS(SP_COMBINE);
       const unsigned Ua = cmb ? att_vtotal(seq, M) : 1u;
       const int cmb_Gq = cmb ? op.att.kv.q_heads / op.att.kv.kv_heads : 1, cmb_nkv = cmb ? op.att.kv.kv_heads : 1;
+      // a K-split slice covers whole heads [h0, h0 + KB / cmb_kbh); a CTA's k-blocks wrap around inside the slice
+      const int cmb_h0 = op.k0 / (cmb_kbh * 64), cmb_hs = KB / cmb_kbh;
       struct CmbPrep { const float* ml; unsigned c_first; int Pn; };
       auto cmb_prep = [&](int pi) -> CmbPrep {
         const SAtt& a = op.att;
         const int m = pi / cmb_nh, hid = pi - m * cmb_nh;
-        const int h = ((kb_first / cmb_kbh) + hid) % a.kv.q_heads, g = h / cmb_Gq, hh = h - g * cmb_Gq;
+        const int h = cmb_h0 + ((kb_first / cmb_kbh) + hid) % cmb_hs, g = h / cmb_Gq, hh = h - g * cmb_Gq;
         unsigned pre = 0;
         for (int mm = 0; mm < m; ++mm) { const unsigned n2 = att_tiles(seq, mm); if (n2) pre += (n2 + ST_ATT_SEGW) * (unsigned)cmb_nkv; }
         const unsigned nt = att_tiles(seq, m);
@@ -970,7 +976,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
         r.o4 = w0 % out4; r.pg = w0 / out4;
         const int m = r.o4 / (count * 16), q = r.o4 - m * (count * 16), jloc = q >> 4, q4 = q & 15;
         int kb = kb_first + jloc; if (kb >= KB) kb -= KB;
-        const int k = kb * 64 + q4 * 4, h = k / ATT_HD(a), d = k - h * ATT_HD(a), g = h / cmb_Gq, hh = h - g * cmb_Gq;
+        const int k = op.k0 + kb * 64 + q4 * 4, h = k / ATT_HD(a), d = k - h * ATT_HD(a), g = h / cmb_Gq, hh = h - g * cmb_Gq;
         r.pi = m * cmb_nh + ((kb_first % cmb_kbh) + jloc) / cmb_kbh;
         r.ap = a.part_acc + ((((size_t)m * cmb_nkv + g) * G) * 8 + hh) * HD + d;             // slot stride 8 * 128 floats
         return r;
@@ -1102,7 +1108,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
           if (((m0 & 6) == 6) || m0 + 2 >= M) {             // flush every 8 rows (s_red holds 8 rows)
             worker_sync();
             const int base = m0 & ~7;
-            if (wt < 8 && base + wt < M) s_inv[base + wt] = rsqrtf((s_red[0][wt] + s_red[1][wt] + s_red[2][wt] + s_red[3][wt]) / (float)K + op.pro_eps);
+            if (wt < 8 && base + wt < M) s_inv[base + wt] = rsqrtf((s_red[0][wt] + s_red[1][wt] + s_red[2][wt] + s_red[3][wt]) / (float)op.krow + op.pro_eps);
             worker_sync();
           }
         }
