@@ -81,8 +81,9 @@ void vv_destroy(vv_ctx* ctx);
  * `data` may be a host or device pointer (cudaMemcpyDefault).  Matrices are stored as bf16,
  * vectors (bias / norm / gamma) as fp32; layouts are repacked for the kernels in
  * vv_finalize_weights (qkv concat, gate/up interleave, conv -> window-GEMV form).
- * Unknown names return VV_ERR_INVALID; names not needed by this path (e.g. acoustic encoder) are
- * accepted and ignored (returns 1). */
+ * Unknown names return VV_ERR_INVALID; names not needed by this path (fix_std, rotary_emb, a tied lm_head) are
+ * accepted and ignored (returns 1).  The acoustic tokenizer encoder is optional: vv_finalize_weights packs it for
+ * vv_voice_encode when all of its tensors were loaded and fails, naming the missing ones, when only some were. */
 int vv_load_tensor(vv_ctx* ctx, const char* name, const void* data, int dtype, const int64_t* shape, int ndim);
 int vv_set_speech_factors(vv_ctx* ctx, float scaling_factor, float bias_factor); /* modeling_vibevoice.py:131-132 */
 int vv_finalize_weights(vv_ctx* ctx);     /* fails with the list of missing tensors */
@@ -156,6 +157,18 @@ int vv_codec_state_reset(vv_ctx* ctx, void* stream);                            
  * so the following vv_lm_decode feeds both streams the same input (:579-581). */
 int vv_frame_tail(vv_ctx* ctx, const float* hidden, const float* noise, const int32_t* active, float cfg_scale,
                   float* latent_out, float* audio_out, float* embeds_inout, void* stream);
+
+/* ---- a-9: voice prompts (modeling_vibevoice_inference.py:149-163, 216-224) ---------------------- *
+ * Non-streaming acoustic tokenizer encoder (modular_vibevoice_tokenizer.py:384-418, 776-813) over n voices of T samples each (the padded
+ * speech_tensors as given), F = ceil(T / 3200) frames per voice; x = mean + sigma[v] * eps; feat = (x + speech_bias) * speech_scale;
+ * acoustic_connector.  sigma is one scale per voice whatever std_dist_type is (gaussian: std_n[v] * fix_std / 0.8, fix: fix_std, none: 0;
+ * eps may then be NULL).  Needs the encoder weights (else VV_ERR_STATE) and at least vv_voice_encode_workspace bytes of 256-byte aligned
+ * device workspace (else VV_ERR_INVALID, nothing launched); a larger workspace processes more voices / rows per pass with the same result.
+ * Outputs: mean_out [n,F,vae_dim] fp32 (optional), embeds_out [n,F,H] fp32. */
+int64_t vv_voice_encode_workspace(vv_ctx* ctx, int n_voices, int64_t n_samples);   /* minimum workspace bytes of the call below */
+int vv_voice_encode(vv_ctx* ctx, const float* wavs /*[n,T] fp32*/, int n, int64_t T, const float* sigma /*[n]*/, const float* eps /*[n,F,vae_dim]*/,
+                    float* mean_out /*[n,F,vae_dim] or NULL*/, float* embeds_out /*[n,F,H] fp32*/, void* workspace, int64_t workspace_bytes,
+                    void* stream);
 
 /* ---- introspection for tests / bench ----------------------------------------------------------- */
 int64_t vv_launch_count(vv_ctx* ctx);     /* kernels launched by this ctx so far */

@@ -7,6 +7,7 @@
 #include "../../include/vibevoice_b200.h"
 #include "vv_kernels.cuh"
 #include "vv_stream.cuh"
+#include "vv_voice.cuh"
 
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -75,6 +76,13 @@ struct Codec {
   StateSeg* segs_dev = nullptr; int n_segs = 0;
   int64_t weight_bytes = 0;
 };
+struct VoiceEnc {           // non-streaming acoustic encoder for voice prompts (a-9); present iff the checkpoint has its tensors
+  bool present = false;
+  std::vector<ConvL> convs;                  // stem, downsample i (before stage i), head: bf16 [Cout][K] tap-major, K = k*Cin rounded up to 8
+  std::vector<std::vector<Block>> stages;    // no streaming state (hist / next stay null)
+  std::vector<int> C;
+  int64_t weight_bytes = 0;
+};
 struct LmLayer { bf16 *wqkv, *wo, *wgu, *wdown; float *bqkv, *ln1, *ln2; };
 struct HeadLayer { bf16 *wgu, *wdown; float* norm; };
 
@@ -102,6 +110,7 @@ struct vv_ctx {
   int sm_count = 132;
   std::map<std::string, RawTensor> raw;
   std::set<std::string> expected;
+  std::set<std::string> voice_expected;      // acoustic encoder tensors: all or none
   std::vector<void*> allocs;
   float speech_scale = NAN, speech_bias = NAN;
   // LM
@@ -118,6 +127,7 @@ struct vv_ctx {
   bf16 *ca_fc1 = nullptr, *ca_fc2 = nullptr, *cs_fc1 = nullptr, *cs_fc2 = nullptr;
   float *ca_b1 = nullptr, *ca_b2 = nullptr, *ca_n = nullptr, *cs_b1 = nullptr, *cs_b2 = nullptr, *cs_n = nullptr;
   Codec dec, enc;
+  VoiceEnc venc;
   int64_t wbytes[6] = {0, 0, 0, 0, 0, 0};
   // KV
   int64_t n_pages = 0; int max_pages = 0; bf16 *kpool = nullptr, *vpool = nullptr;
@@ -677,6 +687,15 @@ static void build_expected(vv_ctx* c) {
     for (int j = 0; j < d.enc_depths[i]; ++j) block_names(e, S("%s.stages.%d.%d", ep.c_str(), i, j));
   }
   for (const char* s : {"head.conv.conv.weight", "head.conv.conv.bias"}) { e.insert(dp + "." + s); e.insert(ep + "." + s); }
+  // the acoustic encoder has the semantic encoder's structure (enc_ratios / enc_depths / enc_n_filters); only its vae_dim differs
+  const std::string ap = "model.acoustic_tokenizer.encoder";
+  auto& v = c->voice_expected;
+  for (int i = 0; i < d.n_stages; ++i) {
+    v.insert(S("%s.downsample_layers.%d.0.conv.conv.weight", ap.c_str(), i));
+    v.insert(S("%s.downsample_layers.%d.0.conv.conv.bias", ap.c_str(), i));
+    for (int j = 0; j < d.enc_depths[i]; ++j) block_names(v, S("%s.stages.%d.%d", ap.c_str(), i, j));
+  }
+  for (const char* s : {"head.conv.conv.weight", "head.conv.conv.bias"}) v.insert(ap + "." + s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -757,8 +776,8 @@ extern "C" int vv_load_tensor(vv_ctx* c, const char* name_, const void* data, in
     (name == "model.speech_scaling_factor" ? c->speech_scale : c->speech_bias) = v;
     return 0;
   }
-  if (!c->expected.count(name)) {
-    if (name.rfind("model.acoustic_tokenizer.encoder.", 0) == 0 || name.find("fix_std") != std::string::npos ||
+  if (!c->expected.count(name) && !c->voice_expected.count(name)) {
+    if (name.find("fix_std") != std::string::npos ||
         name.find("rotary_emb") != std::string::npos || (name == "lm_head.weight" && c->d.tie_word_embeddings))
       return 1;   // not on this path
     return fail(VV_ERR_INVALID, "vv_load_tensor: unknown tensor '%s'", name.c_str());
@@ -856,6 +875,7 @@ static int build_block(vv_ctx* c, const std::string& p, int C, Block* b, int64_t
   RET(take_bf16(c, p + ".ffn.linear2.weight", {C, 4 * C}, &b->w2, bytes));
   RET(take_f32(c, p + ".ffn.linear2.bias", {C}, &b->b2, bytes));
   RET(take_f32(c, p + ".ffn_gamma", {C}, &b->ffn_gamma, bytes));
+  if (!segs) return 0;      // non-streaming use: no conv state
   const int B = c->d.max_batch;
   RET(dmalloc(c, &b->hist, (size_t)B * 6 * C));
   RET(dmalloc(c, &b->next, (size_t)B * 6 * C));
@@ -907,6 +927,51 @@ static int build_convtr(vv_ctx* c, const std::string& p, int Ci, int Co, int s, 
   RET(dmalloc(c, &L_->hist, (size_t)B * Ci));
   RET(dmalloc(c, &L_->next, (size_t)B * Ci));
   segs->push_back({L_->hist, L_->next, Ci});
+  return 0;
+}
+
+// Conv1d [Co][Ci][k] (fp32 or bf16) -> bf16 window-GEMM weight [Co][K], K = k*Ci rounded up to a multiple of 8 with zero columns
+static int build_conv_gemm(vv_ctx* c, const std::string& p, int Ci, int Co, int k, int stride, ConvL* L_, int64_t* bytes) {
+  L_->Cin = Ci; L_->Cout = Co; L_->k = k; L_->stride = stride; L_->ctx = k - stride; L_->N = Co; L_->K = (k * Ci + 7) & ~7;
+  RawTensor* t;
+  RET(need(c, p + ".weight", &t, {Co, Ci, k}));
+  const long long n = (long long)Co * L_->K;
+  RET(dmalloc(c, &L_->w, (size_t)n, false));
+  const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, 65535);
+  if (t->is_f32) repack_conv_pad_kernel<float><<<grid, 256>>>((const float*)t->p, L_->w, Co, Ci, k, L_->K);
+  else repack_conv_pad_kernel<bf16><<<grid, 256>>>((const bf16*)t->p, L_->w, Co, Ci, k, L_->K);
+  CKL();
+  *bytes += (int64_t)Co * Ci * k * 2;
+  RET(take_f32(c, p + ".bias", {Co}, &L_->bias, bytes));
+  return 0;
+}
+
+// acoustic tokenizer encoder (tokenizer.py:694-774) for vv_voice_encode: packed iff the checkpoint has its tensors, all of them
+static int build_voice_encoder(vv_ctx* c) {
+  const auto& d = c->d;
+  std::string missing;
+  int nm = 0;
+  for (auto& n : c->voice_expected) if (!c->raw.count(n)) { if (nm < 8) missing += n + " "; ++nm; }
+  if (nm == (int)c->voice_expected.size()) return 0;
+  if (nm) return fail(VV_ERR_STATE, "acoustic encoder: %d of %zu tensors missing, e.g. %s", nm, c->voice_expected.size(), missing.c_str());
+  if (d.enc_n_filters % 8 || d.hidden_size % 8) return fail(VV_ERR_INVALID, "acoustic encoder: n_filters and hidden size must be multiples of 8");
+  VoiceEnc& v = c->venc;
+  const std::string p = "model.acoustic_tokenizer.encoder";
+  const int ns = d.n_stages, nf = d.enc_n_filters;
+  v.convs.resize(ns + 1); v.stages.resize(ns); v.C.resize(ns);
+  for (int i = 0; i < ns; ++i) {
+    const int C = nf << i;
+    if (i == 0) RET(build_conv_gemm(c, p + ".downsample_layers.0.0.conv.conv", 1, C, 7, 1, &v.convs[0], &v.weight_bytes));
+    else {
+      const int r = d.enc_ratios[ns - 1 - i];     // TokenizerEncoder reverses the ratio list (tokenizer.py:701)
+      RET(build_conv_gemm(c, S("%s.downsample_layers.%d.0.conv.conv", p.c_str(), i), C / 2, C, 2 * r, r, &v.convs[i], &v.weight_bytes));
+    }
+    v.C[i] = C;
+    v.stages[i].resize(d.enc_depths[i]);
+    for (int j = 0; j < d.enc_depths[i]; ++j) RET(build_block(c, S("%s.stages.%d.%d", p.c_str(), i, j), C, &v.stages[i][j], &v.weight_bytes, nullptr));
+  }
+  RET(build_conv_gemm(c, p + ".head.conv.conv", nf << (ns - 1), d.acoustic_vae_dim, 7, 1, &v.convs[ns], &v.weight_bytes));
+  v.present = true;
   return 0;
 }
 
@@ -1155,6 +1220,7 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     RET(upload_segs(c, &k, segs));
     k.weight_bytes = *kb;
   }
+  RET(build_voice_encoder(c));
   max_win = std::max(max_win, (size_t)(hop + 8) * 64);
   RET(dmalloc(c, &c->s_xa, (size_t)B * max_tc));
   RET(dmalloc(c, &c->s_xb, (size_t)B * max_tc));
@@ -2162,6 +2228,160 @@ extern "C" int vv_frame_tail(vv_ctx* c, const float* hidden, const float* noise,
     RET(enqueue_encode(l, audio_out, active, c->s_feat, back));
     return enqueue_connect(l, latent_out, c->s_feat, active, embeds);
   });
+}
+
+// ------------------------------------------------------------------------------------------------
+// a-9 voice prompts: non-streaming acoustic encoder + sampling + acoustic connector (vv_voice_encode)
+// ------------------------------------------------------------------------------------------------
+// Workspace = per-voice activations of one group of voices (two [T_i][C_i] buffers, per-row RMS factors, latent means) + a scratch region
+// S for the GEMM operands of one row chunk.  The minimum holds one voice and 64-row chunks; more workspace means larger groups first,
+// then longer chunks.  Every output row is computed the same way whatever the grouping, so results do not depend on the workspace size.
+struct VoicePlan {
+  std::vector<long long> T;        // rows per voice after conv i (T[0] = samples, T.back() = frames)
+  long long maxTC = 0, F = 0;
+  long long max_bpr = 0;           // largest scratch bytes per row of any GEMM
+};
+static long long align256(long long b) { return (b + 255) & ~255ll; }
+static constexpr long long VOICE_CHUNK_MAX = 65535ll * 64;   // rows of one GEMM launch (grid.y = rows / 64)
+static void voice_plan(const vv_ctx* c, long long T, VoicePlan* pl) {
+  const VoiceEnc& v = c->venc;
+  const int ns = (int)v.stages.size(), H = c->d.hidden_size;
+  pl->T.assign(ns, 0);
+  long long t = T;
+  pl->max_bpr = 8ll * H;                                               // connector: fc1 output + operand planes
+  for (int i = 0; i < ns; ++i) {
+    if (i) t = (t + v.convs[i].stride - 1) / v.convs[i].stride;        // ceil: stride-alignment padding on the right
+    pl->T[i] = t;
+    pl->maxTC = std::max(pl->maxTC, t * v.C[i]);
+    pl->max_bpr = std::max(pl->max_bpr, 32ll * v.C[i]);                // FFN: 4C hidden fp32 + 4C operand planes
+    pl->max_bpr = std::max(pl->max_bpr, 4ll * v.convs[i].K);          // conv: window operand planes
+  }
+  pl->max_bpr = std::max(pl->max_bpr, 4ll * v.convs[ns].K);
+  pl->F = t;
+}
+static long long voice_act_bytes(const vv_ctx* c, const VoicePlan& pl, long long g) {
+  return 2 * align256(g * pl.maxTC * 4) + align256(g * pl.T[0] * 4) + align256(g * pl.F * c->d.acoustic_vae_dim * 4);
+}
+static long long voice_scratch_min(const VoicePlan& pl) { return 64 * pl.max_bpr + 512; }
+static long long voice_chunk(long long S, long long bpr, long long M) {
+  long long R = std::min(((S - 512) / bpr) & ~63ll, VOICE_CHUNK_MAX);
+  return std::min(std::max(R, 64ll), M);
+}
+static int voice_check(vv_ctx* c, int n, int64_t T) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  if (!c->venc.present) return fail(VV_ERR_STATE, "voice encode: the checkpoint has no acoustic tokenizer encoder weights");
+  if (n < 1 || T < 1 || T > (1ll << 30)) return fail(VV_ERR_INVALID, "voice encode: n = %d voices of T = %lld samples out of range", n, (long long)T);
+  return 0;
+}
+
+extern "C" int64_t vv_voice_encode_workspace(vv_ctx* c, int n, int64_t T) {
+  RET(voice_check(c, n, T));
+  VoicePlan pl;
+  voice_plan(c, T, &pl);
+  return voice_act_bytes(c, pl, 1) + voice_scratch_min(pl);
+}
+
+static int voice_gemm(const L& l, const bf16* W, const float* bias, int N, int K, const bf16* hi, const bf16* lo, long long M, float* y, int ldy,
+                      int epi = EPI_NONE, const float* gamma = nullptr) {
+  GemvP p = mk(W, bias, nullptr, K, y, ldy, (int)M, N, K);
+  p.epi = epi;
+  if (epi == EPI_GAMMA_RESID) { p.epi_a = gamma; p.res = y; p.ldres = ldy; }     // in place: the operand is in the planes
+  CK(launch_k(l, gemm_wgmma_kernel, dim3((N + WG_BM - 1) / WG_BM, (unsigned)((M + WG_BN - 1) / WG_BN)), dim3(128), (size_t)WG_SMEM, p, hi, lo));
+  return 0;
+}
+static unsigned ew_grid(const vv_ctx* c, long long n) { return (unsigned)std::max(1ll, std::min((n + 255) / 256, (long long)c->sm_count * 16)); }
+
+// y [nv][T_out][Cout] = causal conv of x [nv][T_in][Cin] (left pad k - s, right stride alignment, both as zeros)
+static int voice_conv(const L& l, const ConvL& cv, const float* x, long long T_in, long long T_out, int nv, float* y, unsigned char* S, long long Sb) {
+  const long long M = nv * T_out, R = voice_chunk(Sb, 4ll * cv.K, M);
+  for (long long m0 = 0; m0 < M; m0 += R) {
+    const long long r = std::min(R, M - m0);
+    bf16* hi = (bf16*)S;
+    bf16* lo = hi + r * cv.K;
+    CK(launch_k(l, voice_window_split_kernel, dim3(ew_grid(l.c, r * cv.K / 4)), dim3(256), 0, x, (int)T_in, (int)T_out, cv.Cin, cv.stride,
+                cv.ctx, cv.k * cv.Cin, cv.K, m0, (int)r, hi, lo));
+    RET(voice_gemm(l, cv.w, cv.bias, cv.Cout, cv.K, hi, lo, r, y + m0 * cv.Cout, cv.Cout));
+  }
+  return 0;
+}
+
+// Block1D over x [nv][T][C] (result back in *x; *y is the other activation buffer)
+static int voice_block(const L& l, const Block& b, float** x, float** y, float* inv, int nv, long long T, unsigned char* S, long long Sb) {
+  const int C = b.C;
+  const float eps = l.c->d.codec_eps;
+  const long long M = nv * T;
+  CK(launch_k(l, voice_rms_kernel, dim3((unsigned)((M + 7) / 8)), dim3(256), 0, (const float*)*x, M, C, eps, inv));
+  CK(launch_k(l, voice_dwconv_kernel, dim3(ew_grid(l.c, M * C)), dim3(256), 0, (const float*)*x, (const float*)inv, (const float*)b.norm_w,
+              (const float*)b.dw_w, (const float*)b.dw_b, (const float*)b.gamma, *y, M, (int)T, C));
+  std::swap(*x, *y);
+  // FFN in row chunks (no halo): norm -> planes -> C x 4C GEMM + GELU -> planes -> 4C x C GEMM, gamma residual in place
+  const long long R = voice_chunk(Sb, 32ll * C, M);
+  float* hid = (float*)S;
+  bf16* planes = (bf16*)(S + align256(R * 16 * C));
+  for (long long m0 = 0; m0 < M; m0 += R) {
+    const long long r = std::min(R, M - m0);
+    float* xr = *x + m0 * C;
+    CK(launch_k(l, voice_norm_split_kernel, dim3((unsigned)((r + 7) / 8)), dim3(256), 0, (const float*)xr, (const float*)b.ffn_norm_w, eps,
+                (int)r, C, planes, planes + r * C));
+    RET(voice_gemm(l, b.w1, b.b1, 4 * C, C, planes, planes + r * C, r, hid, 4 * C, EPI_GELU));
+    CK(launch_k(l, split_bf16_kernel, dim3(ew_grid(l.c, r * C)), dim3(256), 0, (const float*)hid, dense_rows(4 * C), planes, planes + r * 4 * C,
+                (int)r, 4 * C));
+    RET(voice_gemm(l, b.w2, b.b2, C, 4 * C, planes, planes + r * 4 * C, r, xr, C, EPI_GAMMA_RESID, b.ffn_gamma));
+  }
+  return 0;
+}
+
+extern "C" int vv_voice_encode(vv_ctx* c, const float* wavs, int n, int64_t T, const float* sigma, const float* eps, float* mean_out,
+                               float* embeds_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  RET(voice_check(c, n, T));
+  if (!wavs || !embeds_out || !workspace || (eps && !sigma)) return fail(VV_ERR_INVALID, "vv_voice_encode: null argument");
+  if (((uintptr_t)workspace & 255) || ((uintptr_t)eps & 15)) return fail(VV_ERR_INVALID, "vv_voice_encode: workspace must be 256-byte and eps 16-byte aligned");
+  VoicePlan pl;
+  voice_plan(c, T, &pl);
+  const long long smin = voice_scratch_min(pl), need = voice_act_bytes(c, pl, 1) + smin;
+  if (workspace_bytes < need)
+    return fail(VV_ERR_INVALID, "vv_voice_encode: workspace of %lld bytes is below the minimum %lld", (long long)workspace_bytes, need);
+  long long g = n;
+  while (g > 1 && voice_act_bytes(c, pl, g) + smin > workspace_bytes) --g;
+  CK(cudaSetDevice(c->device));
+  CK(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+  const VoiceEnc& v = c->venc;
+  const int ns = (int)v.stages.size(), D = c->d.acoustic_vae_dim, H = c->d.hidden_size;
+  const long long F = pl.F;
+  unsigned char* ws = (unsigned char*)workspace;
+  float* bufA = (float*)ws;
+  float* bufB = (float*)(ws + align256(g * pl.maxTC * 4));
+  float* inv = (float*)(ws + 2 * align256(g * pl.maxTC * 4));
+  float* mean = (float*)(ws + 2 * align256(g * pl.maxTC * 4) + align256(g * pl.T[0] * 4));
+  unsigned char* S = ws + voice_act_bytes(c, pl, g);
+  const long long Sb = workspace_bytes - voice_act_bytes(c, pl, g);
+  L l{c, (cudaStream_t)stream};
+  for (long long v0 = 0; v0 < n; v0 += g) {
+    const int nv = (int)std::min<long long>(g, n - v0);
+    float *x = bufA, *y = bufB;
+    for (int i = 0; i < ns; ++i) {
+      if (i == 0) RET(voice_conv(l, v.convs[0], wavs + v0 * T, T, T, nv, x, S, Sb));
+      else { RET(voice_conv(l, v.convs[i], x, pl.T[i - 1], pl.T[i], nv, y, S, Sb)); std::swap(x, y); }
+      for (const Block& b : v.stages[i]) RET(voice_block(l, b, &x, &y, inv, nv, pl.T[i], S, Sb));
+    }
+    RET(voice_conv(l, v.convs[ns], x, F, F, nv, mean, S, Sb));
+    if (mean_out) CK(cudaMemcpyAsync(mean_out + v0 * F * D, mean, (size_t)nv * F * D * 4, cudaMemcpyDeviceToDevice, l.s));
+    // x = mean + sigma * eps; feat = (x + bias) * scale; acoustic_connector = fc2(RMSNorm_1e-6(fc1(feat)))
+    const long long M = nv * F, R = voice_chunk(Sb, 8ll * H, M);
+    float* y1 = (float*)S;
+    bf16* planes = (bf16*)(S + align256(R * 4 * H));
+    for (long long m0 = 0; m0 < M; m0 += R) {
+      const long long r = std::min(R, M - m0);
+      CK(launch_k(l, voice_sample_split_kernel, dim3(ew_grid(c, r * D / 4)), dim3(256), 0, (const float*)mean, eps ? eps + v0 * F * D : nullptr,
+                  sigma ? sigma + v0 : nullptr, (int)F, D, c->speech_bias, c->speech_scale, m0, (int)r, planes, planes + r * D));
+      RET(voice_gemm(l, c->ca_fc1, c->ca_b1, H, D, planes, planes + r * D, r, y1, H));
+      CK(launch_k(l, voice_norm_split_kernel, dim3((unsigned)((r + 7) / 8)), dim3(256), 0, (const float*)y1, (const float*)c->ca_n, 1e-6f, (int)r, H,
+                  planes, planes + r * H));
+      RET(voice_gemm(l, c->ca_fc2, c->ca_b2, H, H, planes, planes + r * H, r, embeds_out + (v0 * F + m0) * H, H));
+    }
+  }
+  return 0;
 }
 
 struct Rows { int v[16]; };

@@ -142,6 +142,38 @@ class Engine:
         names = ["lm", "head_step", "cond_proj", "decoder", "semantic", "connectors"]
         return {n: int(self.lib.vv_weight_bytes(self.h, i)) for i, n in enumerate(names)}
 
+    # ---- a-9 voice prompts ------------------------------------------------------------------------------
+    def voice_frames(self, n_samples: int) -> int:
+        """latent frames the acoustic encoder makes of `n_samples` (one per hop of prod(ratios) samples, the last one partial)."""
+        hop = int(np.prod(self.config.acoustic_tokenizer_config.encoder_ratios))
+        return -(-int(n_samples) // hop)
+
+    def voice_workspace_bytes(self, n_voices: int, n_samples: int) -> int:
+        """minimum workspace of `voice_encode`; raises if the checkpoint had no acoustic encoder."""
+        return N.check(int(self.lib.vv_voice_encode_workspace(self.h, int(n_voices), int(n_samples))), "vv_voice_encode_workspace")
+
+    def voice_encode(self, wavs: torch.Tensor, sigma: torch.Tensor, eps: Optional[torch.Tensor], mean_out: Optional[torch.Tensor] = None,
+                     workspace_bytes: Optional[int] = None) -> torch.Tensor:
+        """wavs [n, T], sigma [n], eps [n, F, vae_dim] or None -> connected embeddings [n, F, H] fp32 on the device (`vv_voice_encode`).
+        The default workspace fits every voice at once plus 256 MB of GEMM scratch, within 2 GB unless the minimum is larger."""
+        n, T = wavs.shape
+        need = self.voice_workspace_bytes(n, T)
+        ws = int(workspace_bytes) if workspace_bytes is not None else min(need * n + (256 << 20), max(need, 2 << 30))
+        F, H = self.voice_frames(T), self.config.decoder_config.hidden_size
+        cur = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            wavs = wavs.to(self.device, torch.float32).contiguous()
+            sigma = sigma.to(self.device, torch.float32).contiguous()
+            eps = None if eps is None else eps.to(self.device, torch.float32).contiguous()
+            out = torch.empty(n, F, H, dtype=torch.float32, device=self.device)
+            work = torch.empty(max(ws, 1), dtype=torch.uint8, device=self.device)
+            P = lambda t: C.c_void_p(None if t is None else t.data_ptr())
+            N.check(self.lib.vv_voice_encode(self.h, P(wavs), n, T, P(sigma), P(eps), P(mean_out), P(out), P(work), ws, self.s),
+                    "vv_voice_encode")
+        cur.wait_stream(self.stream)
+        return out
+
     # ---- KV -----------------------------------------------------------------------------------------
     def kv_init(self, total_tokens: int):
         pages = (total_tokens + 63) // 64 + 2 * self.B * 2

@@ -145,8 +145,7 @@ class VibeVoiceForConditionalGenerationInference:
         self._torch_prefill = torch_prefill      # keep bf16 LM weights for the PyTorch prompt prefill (prefill.py)
         self._prefill = None
         self._lm_sd: Dict[str, torch.Tensor] = {}
-        self._voice_sd: Dict[str, torch.Tensor] = {}
-        self._voice = None
+        self._voice = None                       # voice-prompt encoder (a-9), set when the checkpoint has the acoustic encoder
         self._scale = self._bias = None
         self._tok = tokenizer_ids
         self._device_index = device
@@ -205,6 +204,7 @@ class VibeVoiceForConditionalGenerationInference:
             self._weights_source = lambda sd=state_dict: iter(sd.items())
         items = state_dict.items() if isinstance(state_dict, dict) else state_dict
         scale = bias = None
+        has_encoder = False
         for name, t in items:
             if name == "model.speech_scaling_factor":
                 scale = float(t); self.model.speech_scaling_factor = torch.tensor(scale)
@@ -212,27 +212,52 @@ class VibeVoiceForConditionalGenerationInference:
                 bias = float(t); self.model.speech_bias_factor = torch.tensor(bias)
             else:
                 eng.load_tensor(name, t)
+                has_encoder |= name.startswith("model.acoustic_tokenizer.encoder.")
                 if self._torch_prefill and name.startswith("model.language_model."):
                     self._lm_sd[name] = t.to(device=eng.device, dtype=torch.bfloat16)
-                elif self._torch_prefill and (name.startswith("model.acoustic_tokenizer.encoder.") or name.startswith("model.acoustic_connector.")):
-                    self._voice_sd[name] = t.to(device=eng.device, dtype=torch.float32)
-        eng.finalize(scale, bias)
+        eng.finalize(scale, bias)          # fails if only part of the acoustic encoder was loaded
         self._scale, self._bias = scale, bias
+        self._voice = self._voice_prompt if has_encoder else None
         if self._torch_prefill:
-            from .prefill import TorchPrefill, TorchVoicePrompt
+            from .prefill import TorchPrefill
             self._prefill = TorchPrefill(self.config, self._lm_sd, eng.device)
-            if any(k.startswith("model.acoustic_tokenizer.encoder.") for k in self._voice_sd):
-                self._voice = TorchVoicePrompt(self.config, self._voice_sd, eng.device)
         return self
+
+    @torch.no_grad()
+    def _voice_prompt(self, speech_tensors: torch.Tensor, speech_masks: torch.Tensor, scale: float, bias: float, noise=None) -> torch.Tensor:
+        """Voice-prompt half of step 0 (`modeling_vibevoice_inference.py:149-163, 216-224`) on the engine (`vv_voice_encode`): acoustic
+        tokenizer encoder over the padded reference wavs, Gaussian sampling (`modular_vibevoice_tokenizer.py:980-989`), (x + bias) * scale,
+        `acoustic_connector`.  -> connected embeddings [sum(speech_masks), H] fp32 on the device, in row-major mask order.  The noise is
+        drawn from the device RNG in the order PyTorch's sampling draws it (std_n [n], then eps [n, F, vae_dim]); `noise=(std_n, eps)`
+        overrides both (tests)."""
+        eng = self.engine
+        if (float(scale), float(bias)) != (self._scale, self._bias):
+            raise ValueError("speech scale / bias (%r, %r) differ from the checkpoint's (%r, %r), which the engine was built with"
+                             % (scale, bias, self._scale, self._bias))
+        tc, dev = self.config.acoustic_tokenizer_config, eng.device
+        wavs = torch.as_tensor(speech_tensors)
+        n, T = wavs.shape
+        shape = (n, eng.voice_frames(T), self.config.acoustic_vae_dim)
+        if tc.std_dist_type == "gaussian":
+            std_n = torch.randn(n, device=dev) if noise is None else noise[0].to(dev, torch.float32)
+            eps = torch.randn(shape, device=dev) if noise is None else noise[1].to(dev, torch.float32)
+            sigma = std_n * (float(tc.fix_std) / 0.8)
+        elif tc.std_dist_type == "fix":
+            eps = torch.randn(shape, device=dev) if noise is None else noise[1].to(dev, torch.float32)
+            sigma = torch.full((n,), float(tc.fix_std), device=dev)
+        else:
+            eps, sigma = None, torch.zeros(n, device=dev)
+        emb = eng.voice_encode(wavs, sigma, eps)
+        return emb[torch.as_tensor(speech_masks).to(dev).bool()]
 
     @classmethod
     def from_pretrained(cls, path: str, torch_dtype=None, device_map=None, attn_implementation=None, tokenizer=None,
                         max_batch: int = 1, **kw):
         """HF checkpoint directory (config.json + *.safetensors), as `demo/inference_from_file.py:295-332` calls it.
         `torch_dtype` / `attn_implementation` are accepted for drop-in compatibility; storage is bf16 and attention is
-        the built-in paged split-KV kernel.  The prompt prefill and the voice-prompt encoder (a-9) are enabled by default, so the
-        demo's `generate(**inputs, is_prefill=True)` works on the returned object; `torch_prefill=False` drops the second (bf16) copy of the
-        LM weights that prefill keeps and leaves only token-by-token prompt ingestion through the decode kernels.
+        the built-in paged split-KV kernel.  The prompt prefill is enabled by default; `torch_prefill=False` drops the second (bf16) copy of
+        the LM weights that prefill keeps and leaves only token-by-token prompt ingestion through the decode kernels.  Voice prompts (the
+        demo's `generate(**inputs, is_prefill=True)` with `speech_tensors`) run on the engine's acoustic encoder either way.
         Special-token ids come from the tokenizer files next to the checkpoint when there are any, else from the public Qwen2.5
         vocabulary (`modular_vibevoice_text_tokenizer.py:175-181`); `generate()` checks them against the tokenizer it is handed."""
         from safetensors import safe_open
@@ -291,7 +316,7 @@ class VibeVoiceForConditionalGenerationInference:
             self.engine.close()
         self.engine = None
         self._prefill = self._voice = None
-        self._lm_sd, self._voice_sd = {}, {}
+        self._lm_sd = {}
         self._kv_tokens = 0
         src = self._weights_source
         self.load_state_dict(transform(src()), self._tok)
@@ -364,9 +389,8 @@ class VibeVoiceForConditionalGenerationInference:
             sample_gen = torch.Generator().manual_seed(torch.initial_seed())
         refresh_negative = bool(kwargs.get("refresh_negative", True))
         use_voice = bool(is_prefill and speech_tensors is not None)
-        if use_voice and (self._voice is None or self._prefill is None):
-            raise N.VVError("voice-prompt prefill needs torch_prefill=True (the from_pretrained default) and the acoustic-encoder weights "
-                            "(a-9 runs on PyTorch library kernels)")
+        if use_voice and self._voice is None:
+            raise N.VVError("voice-prompt prefill needs the acoustic tokenizer encoder weights, which this checkpoint does not have")
         forced: Optional[ForcedTokenScript] = None
         user_procs = []
         if logits_processor is not None:
@@ -461,6 +485,15 @@ class VibeVoiceForConditionalGenerationInference:
         else:
             # ---- prompt prefill through the decode kernel (left-padded rows start late) ----------------------------------
             adv = [0] * B
+            voice_embeds, sim, nxt = None, None, [0] * b
+            if use_voice:         # voice rows take the connected embeddings in mask order, same offsets as above
+                with torch.cuda.stream(eng.stream):
+                    voice_embeds = self._voice(torch.as_tensor(speech_tensors), torch.as_tensor(speech_masks).bool(), self._scale, self._bias,
+                                               noise=kwargs.get("_voice_noise"))
+                sim = torch.as_tensor(speech_input_mask).bool().cpu()
+                counts = sim.sum(dim=-1).tolist()
+                for r in range(1, b):
+                    nxt[r] = nxt[r - 1] + int(counts[r - 1])
             for t in range(Lmax):
                 toks, adv = [], []
                 for r in range(B):
@@ -469,6 +502,12 @@ class VibeVoiceForConditionalGenerationInference:
                     adv.append(1 if live else 0)
                 last = t == Lmax - 1
                 eng.embed_tokens(toks + ([start_id] * B if last else toks), eng.embeds)      # neg rows: [<speech_start>] at pos 0
+                if voice_embeds is not None:
+                    with torch.cuda.stream(eng.stream):
+                        for r in range(b):
+                            if adv[r] and sim[r, t]:
+                                eng.embeds[r].copy_(voice_embeds[nxt[r]])
+                                nxt[r] += 1
                 eng.lm_decode()
                 if not last:
                     eng.kv_commit(adv + [0] * B)
