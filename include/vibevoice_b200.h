@@ -170,7 +170,26 @@ int vv_voice_encode(vv_ctx* ctx, const float* wavs /*[n,T] fp32*/, int n, int64_
                     float* mean_out /*[n,F,vae_dim] or NULL*/, float* embeds_out /*[n,F,H] fp32*/, void* workspace, int64_t workspace_bytes,
                     void* stream);
 
+/* ---- f-2: native prompt prefill (modeling_vibevoice_inference.py:467-482, the prompt half of step 0) ---------------------------- *
+ * All decoder layers over n_tokens prompt rows of ONE sequence at positions [pos0, pos0 + n) on wgmma GEMMs and causal flash attention
+ * (csrc/vv_prefill.cuh).  embeds [n,H] fp32 (device); the rotated K/V are written as bf16 straight into the paged pool (the layout
+ * vv_kv_write uses); attention is causal over everything the sequence holds below pos0 + n, so pos0 > 0 continues a sequence.  Like
+ * vv_kv_write it does not move kv_len (call vv_kv_set_len).  hidden_last [H] fp32 = final-norm hidden state of the last row.
+ * Arithmetic: bf16 GEMM operands, bf16 Q / K / V / P, fp32 accumulators, residual stream and softmax statistics.  Tokens run in chunks of a
+ * multiple of 64 rows sized from the workspace; results are bit-identical for every workspace size.
+ * Errors: workspace below vv_lm_prefill_workspace or not 256-byte aligned -> VV_ERR_INVALID with nothing launched; bad seq, n < 1 or
+ * pos0 + n > max_position_embeddings -> VV_ERR_INVALID; pages cannot be reserved -> VV_ERR_NOMEM; before vv_finalize_weights / vv_kv_init
+ * -> VV_ERR_STATE. */
+int64_t vv_lm_prefill_workspace(vv_ctx* ctx, int64_t n_tokens);          /* minimum workspace bytes of the call below */
+int vv_lm_prefill(vv_ctx* ctx, int seq, int64_t pos0, int64_t n_tokens, const float* embeds, float* hidden_last, void* workspace,
+                  int64_t workspace_bytes, void* stream);
+/* embedding rows of DEVICE token ids (any count; vv_embed_tokens takes at most 16 host ids): out [n,H] fp32; ids outside [0, vocab) give
+ * zero rows. */
+int vv_embed_gather(vv_ctx* ctx, const int32_t* ids_dev, int64_t n, float* out, void* stream);
+
 /* ---- introspection for tests / bench ----------------------------------------------------------- */
+/* the inverse of vv_kv_write: K / V [n][kv_heads][head_dim] bf16 of positions [pos0, pos0 + n) of (seq, layer); either output may be NULL */
+int vv_debug_kv_read(vv_ctx* ctx, int seq, int layer, int64_t pos0, int64_t n, void* k_out, void* v_out, void* stream);
 int64_t vv_launch_count(vv_ctx* ctx);     /* kernels launched by this ctx so far */
 int vv_debug_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, float* y, int M, int N, int K,
                   int prologue, const float* pro_w, float eps, int epilogue, void* stream);

@@ -76,6 +76,10 @@ SYMBOLS = {
     "vv_frame_tail": (_I, [_P, _P, _P, _P, _F, _P, _P, _P, _P]),
     "vv_voice_encode_workspace": (_L, [_P, _I, _L]),
     "vv_voice_encode": (_I, [_P, _P, _I, _L, _P, _P, _P, _P, _P, _L, _P]),
+    "vv_lm_prefill_workspace": (_L, [_P, _L]),
+    "vv_lm_prefill": (_I, [_P, _I, _L, _L, _P, _P, _P, _L, _P]),
+    "vv_embed_gather": (_I, [_P, _P, _L, _P, _P]),
+    "vv_debug_kv_read": (_I, [_P, _I, _I, _L, _L, _P, _P, _P]),
     "vv_launch_count": (_L, [_P]),
     "vv_debug_barrier_bench": (_I, [_P, _I, _I, C.POINTER(C.c_float)]),
     "vv_debug_gemv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _F, _I, _P]),

@@ -8,6 +8,7 @@
 #include "vv_kernels.cuh"
 #include "vv_stream.cuh"
 #include "vv_voice.cuh"
+#include "vv_prefill.cuh"
 
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -2381,6 +2382,138 @@ extern "C" int vv_voice_encode(vv_ctx* c, const float* wavs, int n, int64_t T, c
       RET(voice_gemm(l, c->ca_fc2, c->ca_b2, H, H, planes, planes + r * H, r, embeds_out + (v0 * F + m0) * H, H));
     }
   }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// f-2: native prompt prefill (vv_prefill.cuh).  Workspace = one chunk of R rows (R a multiple of 64): fp32 residual [R][H], operand
+// buffer a1 [R][max(H, nq)] (norm output, attention output) and a2 [R][max(I, nq)] (Q, SwiGLU output), all bf16.  The minimum is one
+// 64-row chunk; a larger workspace takes longer chunks, with the same result.
+// ------------------------------------------------------------------------------------------------
+static long long pf_bytes(const vv_ctx* c, long long R) {
+  const auto& d = c->d;
+  const long long nq = (long long)d.num_q_heads * d.head_dim;
+  return align256(R * 4 * d.hidden_size) + align256(R * 2 * std::max<long long>(d.hidden_size, nq)) +
+         align256(R * 2 * std::max<long long>(d.intermediate_size, nq));
+}
+static int pf_check(vv_ctx* c, int64_t n) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->finalized) return fail(VV_ERR_STATE, "lm prefill: not finalized");
+  if (n < 1) return fail(VV_ERR_INVALID, "lm prefill: n_tokens = %lld must be at least 1", (long long)n);
+  const auto& d = c->d;
+  if (d.head_dim != 64 && d.head_dim != 128) return fail(VV_ERR_INVALID, "lm prefill: head_dim %d (supported: 64, 128)", d.head_dim);
+  if (d.hidden_size % 64 || d.intermediate_size % 64 || (d.num_q_heads * d.head_dim) % 64)
+    return fail(VV_ERR_INVALID, "lm prefill: hidden / intermediate / q widths must be multiples of 64");
+  return 0;
+}
+extern "C" int64_t vv_lm_prefill_workspace(vv_ctx* c, int64_t n_tokens) {
+  RET(pf_check(c, n_tokens));
+  return pf_bytes(c, 64);
+}
+
+extern "C" int vv_lm_prefill(vv_ctx* c, int seq, int64_t pos0, int64_t n, const float* embeds, float* hidden_last, void* workspace,
+                             int64_t workspace_bytes, void* stream) {
+  RET(pf_check(c, n));
+  if (!embeds || !hidden_last || !workspace) return fail(VV_ERR_INVALID, "vv_lm_prefill: null argument");
+  if ((uintptr_t)workspace & 255) return fail(VV_ERR_INVALID, "vv_lm_prefill: workspace must be 256-byte aligned");
+  if (((uintptr_t)embeds & 15) || ((uintptr_t)hidden_last & 15)) return fail(VV_ERR_INVALID, "vv_lm_prefill: embeds / hidden_last must be 16-byte aligned");
+  const long long need = pf_bytes(c, 64);
+  if (workspace_bytes < need)
+    return fail(VV_ERR_INVALID, "vv_lm_prefill: workspace of %lld bytes is below the minimum %lld", (long long)workspace_bytes, need);
+  if (!c->kpool) return fail(VV_ERR_STATE, "vv_lm_prefill: KV pool not initialised (vv_kv_init)");
+  const auto& d = c->d;
+  if (seq < 0 || seq >= 2 * d.max_batch) return fail(VV_ERR_INVALID, "vv_lm_prefill: bad seq %d", seq);
+  if (pos0 < 0 || pos0 + n > d.max_position_embeddings)
+    return fail(VV_ERR_INVALID, "vv_lm_prefill: positions [%lld, %lld) outside [0, %d)", (long long)pos0, (long long)(pos0 + n), d.max_position_embeddings);
+  {
+    const int64_t needp = (pos0 + n + KV_PAGE - 1) / KV_PAGE, have = (int64_t)c->seq_pages[seq].size();
+    if (needp > c->max_pages || needp - have > (int64_t)c->free_pages.size())
+      return fail(VV_ERR_NOMEM, "vv_lm_prefill: KV page pool too small (seq %d needs %lld pages, holds %lld, %lld free)", seq, (long long)needp,
+                  (long long)have, (long long)c->free_pages.size());
+  }
+  CK(cudaSetDevice(c->device));
+  RET(vv_kv_reserve(c, seq, pos0 + n, stream));
+  // rows per chunk: the largest multiple of 64 the workspace holds, at most the prompt (rounded up) and 65535 GEMM row tiles
+  long long R = std::min<long long>((n + 63) & ~63ll, 65535ll * PF_BM);
+  while (R > 64 && pf_bytes(c, R) > workspace_bytes) R -= 64;
+  const int H = d.hidden_size, I = d.intermediate_size, nh = d.num_q_heads, nkv = d.num_kv_heads, hd = d.head_dim, nq = nh * hd;
+  const int Nqkv = nq + 2 * nkv * hd;
+  unsigned char* ws = (unsigned char*)workspace;
+  float* x = (float*)ws;
+  bf16* a1 = (bf16*)(ws + align256(R * 4 * H));
+  bf16* a2 = (bf16*)(ws + align256(R * 4 * H) + align256(R * 2 * std::max(H, nq)));
+  const size_t per_layer = (size_t)c->n_pages * nkv * KV_PAGE * hd;
+  const int* page_row = c->page_table_dev + (size_t)seq * c->max_pages;
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)hd);
+  L l{c, (cudaStream_t)stream};
+  auto gemm = [&](auto kern, const bf16* A, const bf16* W, int M, int N, int K, PfGemm p) -> int {
+    p.A = A; p.W = W; p.M = M; p.N = N; p.K = K;
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PF_SMEM));
+    CK(launch_k(l, kern, dim3((N + PF_BN - 1) / PF_BN, (M + PF_BM - 1) / PF_BM), dim3(256), (size_t)PF_SMEM, p));
+    return 0;
+  };
+  for (long long c0 = 0; c0 < n; c0 += R) {
+    const int r = (int)std::min<long long>(R, n - c0);
+    CK(cudaMemcpyAsync(x, embeds + c0 * H, (size_t)r * H * 4, cudaMemcpyDeviceToDevice, l.s));
+    for (int li = 0; li < d.num_layers; ++li) {
+      const LmLayer& y = c->lm[li];
+      PfGemm p;
+      memset(&p, 0, sizeof p);
+      CK(launch_k(l, pf_rmsnorm_kernel, dim3((r + 7) / 8), dim3(256), 0, (const float*)x, (const float*)y.ln1, d.rms_norm_eps, r, H, a1));
+      p.bias = y.bqkv; p.out = a2; p.ldo = nq; p.kpool = c->kpool + per_layer * li; p.vpool = c->vpool + per_layer * li; p.page_row = page_row;
+      p.nq = nq; p.kv_heads = nkv; p.pos_base = pos0 + c0; p.inv_freq = c->inv_freq;
+      if (hd == 128) RET(gemm(pf_gemm_kernel<PF_EPI_QKV, 128>, a1, y.wqkv, r, Nqkv, H, p));
+      else RET(gemm(pf_gemm_kernel<PF_EPI_QKV, 64>, a1, y.wqkv, r, Nqkv, H, p));
+      const dim3 ag((r + 63) / 64, nh);
+      if (hd == 128) {
+        CK(cudaFuncSetAttribute(pf_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PfAttnCfg<128>::SMEM));
+        CK(launch_k(l, pf_attn_kernel<128>, ag, dim3(128), (size_t)PfAttnCfg<128>::SMEM, (const bf16*)a2, r, nh, nkv, (const bf16*)p.kpool,
+                    (const bf16*)p.vpool, page_row, (long long)(pos0 + c0), scale_log2, a1));
+      } else {
+        CK(cudaFuncSetAttribute(pf_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PfAttnCfg<64>::SMEM));
+        CK(launch_k(l, pf_attn_kernel<64>, ag, dim3(128), (size_t)PfAttnCfg<64>::SMEM, (const bf16*)a2, r, nh, nkv, (const bf16*)p.kpool,
+                    (const bf16*)p.vpool, page_row, (long long)(pos0 + c0), scale_log2, a1));
+      }
+      memset(&p, 0, sizeof p);
+      p.x = x; p.ldx = H;
+      RET(gemm(pf_gemm_kernel<PF_EPI_RESID>, a1, y.wo, r, H, nq, p));
+      CK(launch_k(l, pf_rmsnorm_kernel, dim3((r + 7) / 8), dim3(256), 0, (const float*)x, (const float*)y.ln2, d.rms_norm_eps, r, H, a1));
+      memset(&p, 0, sizeof p);
+      p.out = a2; p.ldo = I;
+      RET(gemm(pf_gemm_kernel<PF_EPI_SWIGLU>, a1, y.wgu, r, 2 * I, H, p));
+      memset(&p, 0, sizeof p);
+      p.x = x; p.ldx = H;
+      RET(gemm(pf_gemm_kernel<PF_EPI_RESID>, a2, y.wdown, r, H, I, p));
+    }
+    if (c0 + r == n) CK(launch_k(l, rows_norm_block_kernel, dim3(1), dim3(256), 0, (const float*)(x + (size_t)(r - 1) * H), (const float*)c->lm_norm, hidden_last, H, d.rms_norm_eps));
+  }
+  return 0;
+}
+
+extern "C" int vv_embed_gather(vv_ctx* c, const int32_t* ids_dev, int64_t n, float* out, void* stream) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->finalized) return fail(VV_ERR_STATE, "vv_embed_gather: not finalized");
+  if (n < 1 || !ids_dev || !out) return fail(VV_ERR_INVALID, "vv_embed_gather: n = %lld ids / null argument", (long long)n);
+  CK(cudaSetDevice(c->device));
+  pf_embed_gather_kernel<<<(unsigned)std::min<int64_t>(n, 65535), 256, 0, (cudaStream_t)stream>>>(c->embed, ids_dev, n, c->d.vocab_size,
+                                                                                                   c->d.hidden_size, out);
+  CKL();
+  c->launches++;
+  return 0;
+}
+
+extern "C" int vv_debug_kv_read(vv_ctx* c, int seq, int layer, int64_t pos0, int64_t n, void* k_out, void* v_out, void* stream) {
+  if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  const auto& d = c->d;
+  if (seq < 0 || seq >= 2 * d.max_batch || layer < 0 || layer >= d.num_layers) return fail(VV_ERR_INVALID, "bad seq %d / layer %d", seq, layer);
+  if (n < 1 || pos0 < 0 || pos0 + n > (int64_t)c->seq_pages[seq].size() * KV_PAGE)
+    return fail(VV_ERR_INVALID, "vv_debug_kv_read: positions [%lld, %lld) outside the reserved range of seq %d", (long long)pos0, (long long)(pos0 + n), seq);
+  const size_t per_layer = (size_t)c->n_pages * d.num_kv_heads * KV_PAGE * d.head_dim;
+  pf_kv_read_kernel<<<(unsigned)std::min<int64_t>(n, 65535), 256, 0, (cudaStream_t)stream>>>(c->kpool + per_layer * layer, c->vpool + per_layer * layer,
+                                                                                              c->page_table_dev + (size_t)seq * c->max_pages, d.num_kv_heads,
+                                                                                              d.head_dim, pos0, n, (bf16*)k_out, (bf16*)v_out);
+  CKL();
+  c->launches++;
   return 0;
 }
 

@@ -174,6 +174,55 @@ class Engine:
         cur.wait_stream(self.stream)
         return out
 
+    # ---- f-2 native prompt prefill ---------------------------------------------------------------------
+    def lm_prefill_workspace_bytes(self, n_tokens: int) -> int:
+        """minimum workspace of `lm_prefill` (one 64-row chunk)."""
+        return N.check(int(self.lib.vv_lm_prefill_workspace(self.h, int(n_tokens))), "vv_lm_prefill_workspace")
+
+    def lm_prefill(self, seq: int, embeds: torch.Tensor, pos0: int = 0, workspace_bytes: Optional[int] = None) -> torch.Tensor:
+        """embeds [n, H] (prompt rows of sequence `seq` at positions pos0..pos0+n) -> final-norm hidden of the last row, fp32 [H] on the device
+        (`vv_lm_prefill`).  K/V land in the paged pool; the caller sets the length with `kv_set_len`.  The default workspace fits the whole
+        prompt in one chunk, within 2 GB unless the minimum is larger (the `voice_encode` rule)."""
+        n = int(embeds.shape[0])
+        need = self.lm_prefill_workspace_bytes(n)
+        ws = int(workspace_bytes) if workspace_bytes is not None else min(need * ((n + 63) // 64), max(need, 2 << 30))
+        cur = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            e = embeds.to(self.device, torch.float32).contiguous()
+            out = torch.empty(self.config.decoder_config.hidden_size, dtype=torch.float32, device=self.device)
+            work = torch.empty(max(ws, 1), dtype=torch.uint8, device=self.device)
+            N.check(self.lib.vv_lm_prefill(self.h, int(seq), int(pos0), n, C.c_void_p(e.data_ptr()), C.c_void_p(out.data_ptr()),
+                                           C.c_void_p(work.data_ptr()), ws, self.s), "vv_lm_prefill")
+        cur.wait_stream(self.stream)
+        return out
+
+    def embed_gather(self, ids) -> torch.Tensor:
+        """token ids (any count) -> embedding rows [n, H] fp32 on the device (`vv_embed_gather`)."""
+        ids = torch.as_tensor(ids).reshape(-1)
+        V = self.config.decoder_config.vocab_size
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= V):
+            raise ValueError("token id outside [0, %d)" % V)
+        cur = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            d = ids.to(self.device, torch.int32).contiguous()
+            out = torch.empty(d.numel(), self.config.decoder_config.hidden_size, dtype=torch.float32, device=self.device)
+            N.check(self.lib.vv_embed_gather(self.h, C.c_void_p(d.data_ptr()), d.numel(), C.c_void_p(out.data_ptr()), self.s), "vv_embed_gather")
+        cur.wait_stream(self.stream)
+        return out
+
+    def kv_read(self, seq: int, layer: int, pos0: int, n: int):
+        """K, V [n, kv_heads, head_dim] bf16 of positions [pos0, pos0 + n) of (seq, layer) (`vv_debug_kv_read`, tests)."""
+        dc = self.config.decoder_config
+        with torch.cuda.stream(self.stream):
+            k = torch.empty(n, dc.num_key_value_heads, dc.head_dim, dtype=torch.bfloat16, device=self.device)
+            v = torch.empty_like(k)
+            N.check(self.lib.vv_debug_kv_read(self.h, int(seq), int(layer), int(pos0), int(n), C.c_void_p(k.data_ptr()), C.c_void_p(v.data_ptr()),
+                                              self.s), "vv_debug_kv_read")
+        self.stream.synchronize()
+        return k, v
+
     # ---- KV -----------------------------------------------------------------------------------------
     def kv_init(self, total_tokens: int):
         pages = (total_tokens + 63) // 64 + 2 * self.B * 2

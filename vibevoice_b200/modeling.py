@@ -140,8 +140,11 @@ class WeightModule:
 
 class VibeVoiceForConditionalGenerationInference:
     def __init__(self, config: VibeVoiceConfig, tokenizer_ids=None, max_batch: int = 1, device: int = 0,
-                 max_diffusion_steps: int = 64, torch_prefill: bool = False):
+                 max_diffusion_steps: int = 64, torch_prefill: bool = False, prefill_impl: Optional[str] = None):
+        if prefill_impl not in (None, "native"):
+            raise ValueError("prefill_impl=%r: the model-level default can only be \"native\" (or None)" % (prefill_impl,))
         self.config = config
+        self._prefill_impl = prefill_impl        # "native": generate() prefills prompts with vv_lm_prefill unless told otherwise
         self._torch_prefill = torch_prefill      # keep bf16 LM weights for the PyTorch prompt prefill (prefill.py)
         self._prefill = None
         self._lm_sd: Dict[str, torch.Tensor] = {}
@@ -256,7 +259,9 @@ class VibeVoiceForConditionalGenerationInference:
         """HF checkpoint directory (config.json + *.safetensors), as `demo/inference_from_file.py:295-332` calls it.
         `torch_dtype` / `attn_implementation` are accepted for drop-in compatibility; storage is bf16 and attention is
         the built-in paged split-KV kernel.  The prompt prefill is enabled by default; `torch_prefill=False` drops the second (bf16) copy of
-        the LM weights that prefill keeps and leaves only token-by-token prompt ingestion through the decode kernels.  Voice prompts (the
+        the LM weights that prefill keeps and leaves only token-by-token prompt ingestion through the decode kernels.  `prefill_impl="native"`
+        makes the engine's own prefill kernels (`vv_lm_prefill`) the default of `generate()`; `torch_prefill` then defaults to False, so no
+        second copy of the LM is kept unless asked for.  Voice prompts (the
         demo's `generate(**inputs, is_prefill=True)` with `speech_tensors`) run on the engine's acoustic encoder either way.
         Special-token ids come from the tokenizer files next to the checkpoint when there are any, else from the public Qwen2.5
         vocabulary (`modular_vibevoice_text_tokenizer.py:175-181`); `generate()` checks them against the tokenizer it is handed."""
@@ -269,7 +274,9 @@ class VibeVoiceForConditionalGenerationInference:
             raise N.VVError("vibevoice_b200 runs on CUDA devices only (device_map=%r); there is no CPU path" % device_map)
         if tokenizer is None:
             tokenizer = cls._tokenizer_ids_from_dir(path, cfg.decoder_config.vocab_size)
-        m = cls(cfg, tokenizer, max_batch=max_batch, device=dev, torch_prefill=bool(kw.pop("torch_prefill", True)))
+        prefill_impl = kw.pop("prefill_impl", None)
+        m = cls(cfg, tokenizer, max_batch=max_batch, device=dev, torch_prefill=bool(kw.pop("torch_prefill", prefill_impl != "native")),
+                prefill_impl=prefill_impl)
 
         def it():
             files = sorted(glob.glob(os.path.join(path, "*.safetensors")))
@@ -369,6 +376,33 @@ class VibeVoiceForConditionalGenerationInference:
         if eng.kv_pages < need_pages:
             eng.kv_init(total_tokens)                                # first call, or a later call that needs more: the pool is re-sized
 
+    def _prefill_rows(self, b, input_ids, attention_mask, lens, use_voice, speech_tensors, speech_masks, speech_input_mask, voice_noise,
+                      gather, run) -> List[torch.Tensor]:
+        """Whole-prompt prefill of rows 0..b-1, one call per row: `gather(ids)` embeds the unpadded ids, the voice embeddings are scattered
+        at `speech_input_mask` (:216-224: acoustic encoder -> sample -> (x+bias)*scale -> connector), `run(r, embeds)` fills the K/V of
+        sequence r and returns its last final-norm hidden state; the row's length is then set.  -> hidden states of the rows."""
+        eng = self.engine
+        hids = []
+        with torch.cuda.stream(eng.stream):
+            voice_embeds = None
+            if use_voice:
+                voice_embeds = self._voice(torch.as_tensor(speech_tensors), torch.as_tensor(speech_masks).bool(), self._scale, self._bias,
+                                           noise=voice_noise)
+                sim = torch.as_tensor(speech_input_mask).bool().cpu()
+                counts = sim.sum(dim=-1).tolist()
+                offs = [0]
+                for c_ in counts:
+                    offs.append(offs[-1] + int(c_))
+            for r in range(b):
+                keep = attention_mask[r].bool()
+                e = gather(input_ids[r][keep])
+                if voice_embeds is not None and counts[r]:
+                    e = e.clone()
+                    e[sim[r][keep].to(e.device)] = voice_embeds[offs[r]:offs[r + 1]].to(e.device, e.dtype)
+                hids.append(run(r, e))
+                eng.kv_set_len(r, int(lens[r]))
+        return hids
+
     @torch.no_grad()
     def generate(self, inputs=None, generation_config=None, logits_processor=None, stopping_criteria=None,
                  prefix_allowed_tokens_fn=None, synced_gpus=None, assistant_model=None, audio_streamer=None,
@@ -451,30 +485,18 @@ class VibeVoiceForConditionalGenerationInference:
 
         lens = init_len.tolist() + [0] * (B - b)
         Lmax = L0
-        use_torch_prefill = self._prefill is not None and kwargs.get("prefill_impl", "auto") != "decode"
-        if use_torch_prefill:
-            # ---- prompt prefill on library kernels (a-9 / f-2), KV handed to the paged pool ------------------------------
-            embw = self._lm_sd["model.language_model.embed_tokens.weight"]
-            hids = []
-            with torch.cuda.stream(eng.stream):
-                voice_embeds = None
-                if use_voice:     # :216-224: acoustic encoder -> sample -> (x+bias)*scale -> connector, scattered at speech_input_mask
-                    voice_embeds = self._voice(torch.as_tensor(speech_tensors), torch.as_tensor(speech_masks).bool(), self._scale, self._bias,
-                                               noise=kwargs.get("_voice_noise"))
-                    sim = torch.as_tensor(speech_input_mask).bool().cpu()
-                    counts = sim.sum(dim=-1).tolist()
-                    offs = [0]
-                    for c_ in counts:
-                        offs.append(offs[-1] + int(c_))
-                for r in range(b):
-                    keep = attention_mask[r].bool()
-                    ids_r = input_ids[r][keep].to(eng.device)
-                    e = embw[ids_r]
-                    if voice_embeds is not None and counts[r]:
-                        e = e.clone()
-                        e[sim[r][keep].to(eng.device)] = voice_embeds[offs[r]:offs[r + 1]].to(e.dtype)
-                    hids.append(self._prefill.run(eng, r, e))
-                    eng.kv_set_len(r, int(lens[r]))
+        impl = kwargs.get("prefill_impl", self._prefill_impl or "auto")
+        use_native_prefill = impl == "native"
+        use_torch_prefill = not use_native_prefill and self._prefill is not None and impl != "decode"
+        if use_torch_prefill or use_native_prefill:
+            # ---- whole-prompt prefill (a-9 / f-2), K/V in the paged pool: library kernels (TorchPrefill) or the engine's (vv_lm_prefill) -----
+            if use_torch_prefill:
+                embw = self._lm_sd["model.language_model.embed_tokens.weight"]
+                gather, run = (lambda ids_r: embw[ids_r.to(eng.device)]), (lambda r, e: self._prefill.run(eng, r, e))
+            else:
+                gather, run = eng.embed_gather, (lambda r, e: eng.lm_prefill(r, e))
+            hids = self._prefill_rows(b, input_ids, attention_mask, lens, use_voice, speech_tensors, speech_masks, speech_input_mask,
+                                      kwargs.get("_voice_noise"), gather, run)
             eng.embed_tokens([pad_tok] * B + [start_id] * B, eng.embeds)     # negative rows: [<speech_start>] at pos 0 (:379-386)
             eng.lm_decode()
             with torch.cuda.stream(eng.stream):
