@@ -11,9 +11,8 @@
 //                                     transformers Qwen2RMSNorm (modeling_qwen2.py:249-266)
 //   gemv epilogues SWIGLU/GATED_RESID modular_vibevoice_diffusion_head.py:116-123, 158-161
 //   gemv epilogues GELU/GAMMA_RESID   modular_vibevoice_tokenizer.py:592-596, 670-682
-//   rope_append / attn_*              transformers Qwen2Attention (modeling_qwen2.py:116-174)
-//   dpm_update_proj                   modeling_vibevoice_inference.py:703-709 + schedule/dpm_solver.py:581-584, 669-677, 738-764
 //   assemble_window / dwconv_res      modular_vibevoice_tokenizer.py:327-382 (streaming SConv1d), 786-794
+// (decode attention and the DPM-Solver++ update run only inside the weight-stream kernel: anchors at SAtt / SDpm in vv_stream.cuh)
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -986,12 +985,6 @@ __global__ void advance_kernel(const StateSeg* __restrict__ segs, const int* __r
   const float* a = s.next + (size_t)b * s.n;
   for (int i = blockIdx.z * blockDim.x + threadIdx.x; i < s.n; i += gridDim.z * blockDim.x) d[i] = a[i];
 }
-__global__ void state_zero_kernel(const StateSeg* __restrict__ segs, const int* __restrict__ rows) {
-  const int b = rows[blockIdx.y];
-  const StateSeg s = segs[blockIdx.x];
-  float* d = s.hist + (size_t)b * s.n;
-  for (int i = threadIdx.x; i < s.n; i += blockDim.x) d[i] = 0.f;
-}
 
 // ---------------------------------------------------------------------------------------------
 // LLM decode step pieces
@@ -1008,388 +1001,11 @@ struct KvView {
   int kv_heads, q_heads;
 };
 
-// qkv [M, (q_heads + 2 kv_heads) * HD] fp32 (bias added) -> q_rot fp32, K/V (bf16) appended at kv_len[m]
-__global__ void rope_append_kernel(const float* __restrict__ qkv, float* __restrict__ q_rot, KvView kv,
-                                   const float* __restrict__ inv_freq /*[HD/2]*/) {
-  pdl_trigger();
-  pdl_wait();
-  const int m = blockIdx.x;
-  if (!kv.row_mode[m]) return;
-  const int pos = kv.kv_len[m];
-  const int nq = kv.q_heads, nkv = kv.kv_heads;
-  const float* row = qkv + (size_t)m * (nq + 2 * nkv) * HD;
-  const int page = kv.page_table[(size_t)m * kv.max_pages + pos / KV_PAGE];
-  const int slot = pos % KV_PAGE;
-  for (int i = threadIdx.x; i < (nq + nkv) * (HD / 2); i += blockDim.x) {
-    const int h = i / (HD / 2), d = i % (HD / 2);
-    const float ang = (float)pos * inv_freq[d];
-    float sn, cs;
-    sincosf(ang, &sn, &cs);
-    const float x1 = row[h * HD + d], x2 = row[h * HD + d + HD / 2];
-    const float o1 = x1 * cs - x2 * sn, o2 = x2 * cs + x1 * sn;
-    if (h < nq) {
-      q_rot[((size_t)m * nq + h) * HD + d] = o1;
-      q_rot[((size_t)m * nq + h) * HD + d + HD / 2] = o2;
-    } else {
-      bf16* kp = kv.kpool + (((size_t)page * nkv + (h - nq)) * KV_PAGE + slot) * HD;
-      kp[d] = __float2bfloat16_rn(o1);
-      kp[d + HD / 2] = __float2bfloat16_rn(o2);
-    }
-  }
-  for (int i = threadIdx.x; i < nkv * HD; i += blockDim.x) {
-    const int h = i / HD, d = i % HD;
-    bf16* vp = kv.vpool + (((size_t)page * nkv + h) * KV_PAGE + slot) * HD;
-    vp[d] = __float2bfloat16_rn(row[(nq + nkv + h) * HD + d]);
-  }
-}
-
-// split-KV partial attention: CTA = (split, kv head, sequence); 4 warps; 32-token K/V tiles double-buffered in
-// shared memory with cp.async so the next tile streams from HBM while the current one is being consumed.
-constexpr int ATT_TILE = 32;
 constexpr int ATT_MAXG = 8;     // q heads per kv head (6 for 1.5B, 7 for 7B)
-__global__ void __launch_bounds__(128) attn_partial_kernel(const float* __restrict__ q_rot, KvView kv, float* __restrict__ part_acc,
-                                                           float* __restrict__ part_ml, int nsplit, float scale) {
-  pdl_trigger();
-  pdl_wait();
-  const int s = blockIdx.x, g = blockIdx.y, m = blockIdx.z;
-  if (!kv.row_mode[m]) return;
-  const int G = kv.q_heads / kv.kv_heads;
-  const int L = kv.kv_len[m] + 1;
-  const int ntiles = (L + ATT_TILE - 1) / ATT_TILE;
-  const int tps = (ntiles + nsplit - 1) / nsplit;
-  const int t_begin = s * tps, t_end = min(ntiles, (s + 1) * tps);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-  __shared__ __align__(16) bf16 Ks[2][ATT_TILE][HD + 8];
-  __shared__ __align__(16) bf16 Vs[2][ATT_TILE][HD + 8];
-  __shared__ __align__(16) float qs[ATT_MAXG][HD];
-  __shared__ float ps[ATT_MAXG][ATT_TILE];
-
-  auto prefetch = [&](int t, int buf) {
-    const int tok0 = t * ATT_TILE;
-    const int page = kv.page_table[(size_t)m * kv.max_pages + tok0 / KV_PAGE];
-    const size_t base = (((size_t)page * kv.kv_heads + g) * KV_PAGE + (tok0 % KV_PAGE)) * HD;
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const int idx = tid + it * 128;
-      const int r = idx >> 4, c = (idx & 15) * 8;
-      cp_async16(&Ks[buf][r][c], kv.kpool + base + (size_t)r * HD + c, 16);
-      cp_async16(&Vs[buf][r][c], kv.vpool + base + (size_t)r * HD + c, (tok0 + r < L) ? 16 : 0);   // zero-fill beyond the sequence
-    }
-  };
-  if (t_begin < t_end) prefetch(t_begin, 0);
-  cp_async_commit();
-  for (int i = tid; i < G * HD; i += 128) qs[i / HD][i % HD] = q_rot[((size_t)m * kv.q_heads + g * G) * HD + i];
-
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-
-  for (int t = t_begin; t < t_end; ++t) {
-    const int buf = (t - t_begin) & 1;
-    const int tok0 = t * ATT_TILE;
-    if (t + 1 < t_end) prefetch(t + 1, buf ^ 1);
-    cp_async_commit();
-    cp_async_wait<1>();
-    __syncthreads();
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int h = warp + 4 * hh;
-      if (h >= G) continue;
-      float sc = 0.f;
-#pragma unroll
-      for (int c = 0; c < HD; c += 8) {
-        float kf[8];
-        bf16x8_unpack(*reinterpret_cast<const uint4*>(&Ks[buf][lane][c]), kf);
-        const float4 qa = *reinterpret_cast<const float4*>(&qs[h][c]);
-        const float4 qb = *reinterpret_cast<const float4*>(&qs[h][c + 4]);
-        sc = fmaf(kf[0], qa.x, sc); sc = fmaf(kf[1], qa.y, sc); sc = fmaf(kf[2], qa.z, sc); sc = fmaf(kf[3], qa.w, sc);
-        sc = fmaf(kf[4], qb.x, sc); sc = fmaf(kf[5], qb.y, sc); sc = fmaf(kf[6], qb.z, sc); sc = fmaf(kf[7], qb.w, sc);
-      }
-      sc = (tok0 + lane < L) ? sc * scale : -INFINITY;
-      const float mt = warp_max(sc);
-      const float mn = fmaxf(m_run[hh], mt);           // finite: every tile in range has >= 1 valid token
-      const float pj = __expf(sc - mn);
-      const float corr = __expf(m_run[hh] - mn);        // exp(-inf) = 0 on the first tile
-      l_run[hh] = l_run[hh] * corr + warp_sum(pj);
-      m_run[hh] = mn;
-      ps[h][lane] = pj;
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 4; ++j) acc[hh][j] *= corr;
-#pragma unroll 8
-      for (int tt = 0; tt < ATT_TILE; ++tt) {
-        const float pv = ps[h][tt];
-        const uint2 v2 = *reinterpret_cast<const uint2*>(&Vs[buf][tt][lane * 4]);
-        acc[hh][0] = fmaf(pv, __uint_as_float(v2.x << 16), acc[hh][0]);
-        acc[hh][1] = fmaf(pv, __uint_as_float(v2.x & 0xffff0000u), acc[hh][1]);
-        acc[hh][2] = fmaf(pv, __uint_as_float(v2.y << 16), acc[hh][2]);
-        acc[hh][3] = fmaf(pv, __uint_as_float(v2.y & 0xffff0000u), acc[hh][3]);
-      }
-      __syncwarp();
-    }
-    __syncthreads();    // everyone is done with `buf` before the prefetch of tile t+2 overwrites it
-  }
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    const int h = warp + 4 * hh;
-    if (h >= G) continue;
-    const size_t o = ((size_t)m * kv.q_heads + g * G + h) * nsplit + s;
-    float4 a = make_float4(acc[hh][0], acc[hh][1], acc[hh][2], acc[hh][3]);
-    *reinterpret_cast<float4*>(part_acc + o * HD + lane * 4) = a;
-    if (lane == 0) { part_ml[o * 2] = m_run[hh]; part_ml[o * 2 + 1] = l_run[hh]; }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Tensor-core split-KV partial attention (mma.sync m16n8k16, bf16 operands, fp32 accumulate).
-// The scalar kernel above is issue-bound (~1300 warp instructions per 32-token tile); here a warp needs ~110
-// per 16 tokens.  GQA trick: the 16 rows of the MMA "M" dimension hold the G <= 8 query heads of one KV group
-// TWICE -- rows 0..7 the bf16 high parts, rows 8..15 the bf16 low parts (q = hi + lo to 2^-16) -- so a single
-// MMA yields hi*K and lo*K, summed in registers; the same packing carries P = hi + lo through the P*V product.
-// CTA = 4 warps over 64-token K/V tiles (cp.async double-buffered); warp w owns tokens [16w, 16w+16) of every tile
-// with its own online-softmax state, merged through shared memory at the end.
-// ---------------------------------------------------------------------------------------------
-constexpr int AT2_TILE = 64, AT2_LD = HD + 8;
-constexpr int AT2_SMEM = 4 * AT2_TILE * AT2_LD * 2 + 16 * AT2_LD * 2 + 2 * HD * 2;
+constexpr int AT2_LD = HD + 8;  // row stride (bf16) of the stream kernel's attention Q tile: +8 = 16 B pad, ldmatrix conflict-free
 VV_DEVINL void ldmatrix_x4_trans(unsigned (&r)[4], const void* smem) {
   unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(sa));
-}
-// `fused_rope`: q_src is the raw QKV projection [M, (nq+2nkv)*HD] (bias added); RoPE of q is applied while staging Q, and the
-// split that owns the newest token rotates k, rounds K/V to bf16, stores them into the paged pool and splices them into its
-// shared-memory tile (replaces rope_append_kernel: one launch and one q round trip less per layer).
-__global__ void __launch_bounds__(128) attn_partial_mma_kernel(const float* __restrict__ q_src, int fused_rope, const float* __restrict__ inv_freq,
-                                                               KvView kv, float* __restrict__ part_acc, float* __restrict__ part_ml, int nsplit,
-                                                               float scale) {
-  pdl_trigger();
-  pdl_wait();
-  extern __shared__ __align__(16) unsigned char at_smem[];
-  typedef bf16 (*TileP)[AT2_TILE][AT2_LD];
-  TileP Ks = reinterpret_cast<TileP>(at_smem);
-  TileP Vs = reinterpret_cast<TileP>(at_smem + 2 * AT2_TILE * AT2_LD * 2);
-  bf16 (*Qs)[AT2_LD] = reinterpret_cast<bf16 (*)[AT2_LD]>(at_smem + 4 * AT2_TILE * AT2_LD * 2);
-  bf16* knew = reinterpret_cast<bf16*>(at_smem + 4 * AT2_TILE * AT2_LD * 2 + 16 * AT2_LD * 2);
-  bf16* vnew = knew + HD;
-  const int s = blockIdx.x, g = blockIdx.y, m = blockIdx.z;
-  if (!kv.row_mode[m]) return;
-  const int G = kv.q_heads / kv.kv_heads;
-  const int pos = kv.kv_len[m];
-  const int L = pos + 1;
-  const int ntiles = (L + AT2_TILE - 1) / AT2_TILE;
-  const int tps = (ntiles + nsplit - 1) / nsplit;
-  const int t_begin = s * tps, t_end = min(ntiles, (s + 1) * tps);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const size_t obase = ((size_t)m * kv.q_heads + g * G) * nsplit + s;        // + h * nsplit per head
-  if (t_begin >= t_end) {                                                   // empty split: neutral partial
-    for (int i = tid; i < G * HD; i += 128) part_acc[(obase + (size_t)(i / HD) * nsplit) * HD + (i % HD)] = 0.f;
-    if (tid < G) { part_ml[(obase + (size_t)tid * nsplit) * 2] = -INFINITY; part_ml[(obase + (size_t)tid * nsplit) * 2 + 1] = 0.f; }
-    return;
-  }
-  auto prefetch = [&](int t, int buf) {
-    const int tok0 = t * AT2_TILE;
-    const int page = kv.page_table[(size_t)m * kv.max_pages + tok0 / KV_PAGE];
-    const size_t base = (((size_t)page * kv.kv_heads + g) * KV_PAGE + (tok0 % KV_PAGE)) * HD;
-#pragma unroll
-    for (int it = 0; it < 8; ++it) {
-      const int idx = tid + it * 128;
-      const int r = idx >> 4, c = (idx & 15) * 8;
-      cp_async16(&Ks[buf][r][c], kv.kpool + base + (size_t)r * HD + c, 16);
-      cp_async16(&Vs[buf][r][c], kv.vpool + base + (size_t)r * HD + c, (tok0 + r < L) ? 16 : 0);
-    }
-  };
-  prefetch(t_begin, 0);
-  cp_async_commit();
-  // Q: rows 0..7 = hi(q*scale) of heads 0..G-1, rows 8..15 = lo
-  const bool owner = fused_rope && (ntiles - 1 >= t_begin) && (ntiles - 1 < t_end);
-  if (!fused_rope) {
-    for (int i = tid; i < 8 * HD; i += 128) {
-      const int h = i / HD, d = i % HD;
-      const float v = (h < G) ? q_src[((size_t)m * kv.q_heads + g * G + h) * HD + d] * scale : 0.f;
-      const bf16 hi = __float2bfloat16_rn(v);
-      Qs[h][d] = hi;
-      Qs[h + 8][d] = __float2bfloat16_rn(v - __bfloat162float(hi));
-    }
-  } else {
-    const float* row = q_src + (size_t)m * (kv.q_heads + 2 * kv.kv_heads) * HD;
-    for (int i = tid; i < 8 * (HD / 2); i += 128) {
-      const int h = i / (HD / 2), d = i % (HD / 2);
-      float o1 = 0.f, o2 = 0.f;
-      if (h < G) {
-        float sn, cs;
-        sincosf((float)pos * inv_freq[d], &sn, &cs);
-        const float x1 = row[(g * G + h) * HD + d], x2 = row[(g * G + h) * HD + d + HD / 2];
-        o1 = (x1 * cs - x2 * sn) * scale;
-        o2 = (x2 * cs + x1 * sn) * scale;
-      }
-      const bf16 h1 = __float2bfloat16_rn(o1), h2 = __float2bfloat16_rn(o2);
-      Qs[h][d] = h1; Qs[h][d + HD / 2] = h2;
-      Qs[h + 8][d] = __float2bfloat16_rn(o1 - __bfloat162float(h1));
-      Qs[h + 8][d + HD / 2] = __float2bfloat16_rn(o2 - __bfloat162float(h2));
-    }
-    if (owner) {
-      const int page = kv.page_table[(size_t)m * kv.max_pages + pos / KV_PAGE];
-      const size_t oo = (((size_t)page * kv.kv_heads + g) * KV_PAGE + (pos % KV_PAGE)) * HD;
-      if (tid < HD / 2) {
-        const int d = tid;
-        float sn, cs;
-        sincosf((float)pos * inv_freq[d], &sn, &cs);
-        const float x1 = row[(kv.q_heads + g) * HD + d], x2 = row[(kv.q_heads + g) * HD + d + HD / 2];
-        const bf16 k1 = __float2bfloat16_rn(x1 * cs - x2 * sn), k2 = __float2bfloat16_rn(x2 * cs + x1 * sn);
-        knew[d] = k1; knew[d + HD / 2] = k2;
-        kv.kpool[oo + d] = k1; kv.kpool[oo + d + HD / 2] = k2;
-      } else {
-        for (int d = tid - HD / 2; d < HD; d += 64) {
-          const bf16 vv_ = __float2bfloat16_rn(row[(kv.q_heads + kv.kv_heads + g) * HD + d]);
-          vnew[d] = vv_;
-          kv.vpool[oo + d] = vv_;
-        }
-      }
-    }
-  }
-  __syncthreads();
-  unsigned qa[8][4];
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks) ldmatrix_x4(qa[ks], &Qs[lane & 15][ks * 16 + (lane >> 4) * 8]);
-  float o[16][4];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) { o[i][0] = 0.f; o[i][1] = 0.f; o[i][2] = 0.f; o[i][3] = 0.f; }
-  float m_run = -INFINITY, l_run = 0.f;
-
-  for (int t = t_begin; t < t_end; ++t) {
-    const int buf = (t - t_begin) & 1;
-    const int tok0 = t * AT2_TILE;
-    if (t + 1 < t_end) prefetch(t + 1, buf ^ 1);
-    cp_async_commit();
-    cp_async_wait<1>();
-    __syncthreads();
-    if (owner && t == ntiles - 1) {              // splice the fresh K/V row over whatever the pool held when the tile was fetched
-      Ks[buf][pos - tok0][tid] = knew[tid];
-      Vs[buf][pos - tok0][tid] = vnew[tid];
-      __syncthreads();
-    }
-    float sa[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      unsigned kb[4];
-      ldmatrix_x4(kb, &Ks[buf][warp * 16 + (lane & 7) + ((lane >> 4) << 3)][ks * 16 + ((lane >> 3) & 1) * 8]);
-      mma_bf16_16816(sa[0], qa[ks], kb[0], kb[1]);
-      mma_bf16_16816(sa[1], qa[ks], kb[2], kb[3]);
-    }
-    // head = lane/4; this lane holds tokens tb+{0,1} (n-tile 0) and tb+{8,9} (n-tile 1); hi-row + lo-row
-    const int tb = tok0 + warp * 16 + (lane & 3) * 2;
-    float sv[4] = {sa[0][0] + sa[0][2], sa[0][1] + sa[0][3], sa[1][0] + sa[1][2], sa[1][1] + sa[1][3]};
-    if (tb >= L) sv[0] = -INFINITY;
-    if (tb + 1 >= L) sv[1] = -INFINITY;
-    if (tb + 8 >= L) sv[2] = -INFINITY;
-    if (tb + 9 >= L) sv[3] = -INFINITY;
-    float mt = fmaxf(fmaxf(sv[0], sv[1]), fmaxf(sv[2], sv[3]));
-    mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
-    mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
-    const float mn = fmaxf(m_run, mt);
-    const float msafe = (mn == -INFINITY) ? 0.f : mn;
-    float pv[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) pv[i] = __expf(sv[i] - msafe);
-    const float corr = __expf(m_run - msafe);
-    float rs = pv[0] + pv[1] + pv[2] + pv[3];
-    rs += __shfl_xor_sync(0xffffffffu, rs, 1);
-    rs += __shfl_xor_sync(0xffffffffu, rs, 2);
-    l_run = l_run * corr + rs;
-    m_run = mn;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) { o[i][0] *= corr; o[i][1] *= corr; o[i][2] *= corr; o[i][3] *= corr; }
-    float ph[4], pl[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { ph[i] = __bfloat162float(__float2bfloat16_rn(pv[i])); pl[i] = pv[i] - ph[i]; }
-    unsigned pa[4] = {pack_bf16(ph[0], ph[1]), pack_bf16(pl[0], pl[1]), pack_bf16(ph[2], ph[3]), pack_bf16(pl[2], pl[3])};
-#pragma unroll
-    for (int np = 0; np < 8; ++np) {
-      unsigned vb[4];
-      ldmatrix_x4_trans(vb, &Vs[buf][warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8][np * 16 + (lane >> 4) * 8]);
-      mma_bf16_16816(o[2 * np], pa, vb[0], vb[1]);
-      mma_bf16_16816(o[2 * np + 1], pa, vb[2], vb[3]);
-    }
-    __syncthreads();
-  }
-  cp_async_wait<0>();
-  __syncthreads();
-  // merge the 4 warps' partial (m, l, O) through shared memory (K/V buffers are free now)
-  float* mo = reinterpret_cast<float*>(at_smem);            // [4][8][HD]
-  float* mlw = mo + 4 * 8 * HD;                             // [4][8][2]
-  const int h = lane >> 2;
-#pragma unroll
-  for (int nt = 0; nt < 16; ++nt) {
-    const int d = nt * 8 + (lane & 3) * 2;
-    mo[(warp * 8 + h) * HD + d] = o[nt][0] + o[nt][2];
-    mo[(warp * 8 + h) * HD + d + 1] = o[nt][1] + o[nt][3];
-  }
-  if ((lane & 3) == 0) { mlw[(warp * 8 + h) * 2] = m_run; mlw[(warp * 8 + h) * 2 + 1] = l_run; }
-  __syncthreads();
-  for (int hh = 0; hh < G; ++hh) {
-    float mx = -INFINITY;
-#pragma unroll
-    for (int w = 0; w < 4; ++w) mx = fmaxf(mx, mlw[(w * 8 + hh) * 2]);
-    float num = 0.f, den = 0.f;
-#pragma unroll
-    for (int w = 0; w < 4; ++w) {
-      const float mw = mlw[(w * 8 + hh) * 2];
-      const float wgt = (mw == -INFINITY) ? 0.f : __expf(mw - mx);
-      num = fmaf(wgt, mo[(w * 8 + hh) * HD + tid], num);
-      den = fmaf(wgt, mlw[(w * 8 + hh) * 2 + 1], den);
-    }
-    const size_t oo = obase + (size_t)hh * nsplit;
-    part_acc[oo * HD + tid] = num;
-    if (tid == 0) { part_ml[oo * 2] = mx; part_ml[oo * 2 + 1] = den; }
-  }
-}
-
-// merge the split partials: weights computed once per (row, head) in shared memory; warp w accumulates splits s = w (mod 4)
-// with one float4 (4 dims) per lane, the four warp sums are added through shared memory.
-__global__ void __launch_bounds__(128) attn_combine_kernel(const float* __restrict__ part_acc, const float* __restrict__ part_ml,
-                                                           const int* __restrict__ row_mode, float* __restrict__ out, int q_heads,
-                                                           int nsplit) {
-  pdl_trigger();
-  pdl_wait();
-  const int h = blockIdx.x, m = blockIdx.y, d = threadIdx.x, lane = d & 31, warp = d >> 5;
-  if (!row_mode[m]) return;
-  const size_t o = ((size_t)m * q_heads + h) * nsplit;
-  __shared__ float wsh[512];
-  __shared__ float red[4];
-  __shared__ __align__(16) float part[4][HD];
-  float mx = -INFINITY;
-  for (int s = d; s < nsplit; s += 128) mx = fmaxf(mx, part_ml[(o + s) * 2]);
-  mx = warp_max(mx);
-  if (lane == 0) red[warp] = mx;
-  __syncthreads();
-  mx = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
-  __syncthreads();
-  float den = 0.f;
-  for (int s = d; s < nsplit; s += 128) {
-    const float ms = part_ml[(o + s) * 2];
-    const float w = (ms == -INFINITY) ? 0.f : __expf(ms - mx);
-    wsh[s] = w;
-    den = fmaf(w, part_ml[(o + s) * 2 + 1], den);
-  }
-  den = warp_sum(den);
-  if (lane == 0) red[warp] = den;
-  __syncthreads();
-  den = red[0] + red[1] + red[2] + red[3];
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 4
-  for (int s = warp; s < nsplit; s += 4) {
-    const float w = wsh[s];
-    const float4 v = *reinterpret_cast<const float4*>(part_acc + (o + s) * HD + lane * 4);
-    acc.x = fmaf(w, v.x, acc.x); acc.y = fmaf(w, v.y, acc.y); acc.z = fmaf(w, v.z, acc.z); acc.w = fmaf(w, v.w, acc.w);
-  }
-  *reinterpret_cast<float4*>(&part[warp][lane * 4]) = acc;
-  __syncthreads();
-  out[((size_t)m * q_heads + h) * HD + d] = (part[0][d] + part[1][d] + part[2][d] + part[3][d]) / den;
-}
-
-__global__ void embed_gather_kernel(const bf16* __restrict__ table, const int* __restrict__ tokens, float* __restrict__ out, int H) {
-  const int r = blockIdx.x;
-  const bf16* row = table + (size_t)tokens[r] * H;
-  for (int k = threadIdx.x; k < H; k += blockDim.x) out[(size_t)r * H + k] = __bfloat162float(row[k]);
 }
 
 // logits over the valid ids + constrained argmax (VibeVoiceTokenConstraintProcessor + argmax, :53-66, :498)
@@ -1424,11 +1040,6 @@ __global__ void __launch_bounds__(256) lm_head_argmax_kernel(const float* __rest
   }
 }
 
-__global__ void kv_commit_kernel(int* __restrict__ kv_len, const int* __restrict__ advance, int n) {
-  const int i = threadIdx.x;
-  if (i < n) kv_len[i] += advance[i];
-}
-
 // ---------------------------------------------------------------------------------------------
 // diffusion sampler glue
 // ---------------------------------------------------------------------------------------------
@@ -1445,65 +1056,8 @@ __global__ void head_cond_prep_kernel(const float* __restrict__ condp, const flo
   c_all[idx] = silu_f(condp[(size_t)r * H + k] + temb[(size_t)i * H + k]);
 }
 
-struct DpmCoef { float a0, s0, ks, kx, rinv; int order; float kn; };   // kn: per-step noise gain (sde-dpmsolver++), 0 for the ODE solver
-
-// Step `i` CFG + DPM-Solver++(2M) update of z from the head output v of step i, then (optionally)
-// the projection x = noisy_images_proj(z') for the next head evaluation, rows b and B+b.
-//   v = v_u + s (v_c - v_u); x0 = a0 z - s0 v; z' = ks z - kx x0 [- 0.5 kx rinv (x0 - x0_prev)] [+ kn * step_noise[step]]
-// (sde-dpmsolver++, dpm_solver.py:680-686 / 785-793: same two forms with other ks/kx plus the variance-noise term; step_noise is
-//  [n_steps][B][64] or nullptr for the ODE solver)
-// grid (B, H/256): every CTA recomputes the 64-element update from the read-only (z_in, x0_in) pair,
-// CTA y==0 publishes (z_out, x0_out); the ping-pong removes the cross-CTA read/write hazard.
-__global__ void __launch_bounds__(256) dpm_update_proj_kernel(const float* __restrict__ z_in, float* __restrict__ z_out,
-                                                              const float* __restrict__ x0_in, float* __restrict__ x0_out,
-                                                              const float* __restrict__ v, const float* __restrict__ noise,
-                                                              const DpmCoef* __restrict__ coef, int step, const float* __restrict__ cfg_p,
-                                                              const bf16* __restrict__ w_noisy /*[H][64]*/, float* __restrict__ xout,
-                                                              float* __restrict__ latent_out, int B, int H, int do_proj,
-                                                              const float* __restrict__ step_noise) {
-  pdl_trigger();
-  pdl_wait();
-  const int b = blockIdx.x, tid = threadIdx.x;
-  __shared__ float zs[64];
-  if (tid < 64) {
-    float zn, x0 = 0.f;
-    if (step < 0) {
-      zn = noise[b * 64 + tid];                           // z_0 = CPU-RNG noise (:701)
-    } else {
-      const DpmCoef c = coef[step];
-      const float cfg = *cfg_p;
-      const float vc = v[(size_t)b * 64 + tid], vu = v[(size_t)(B + b) * 64 + tid];
-      const float vv = vu + cfg * (vc - vu);
-      const float zo = z_in[b * 64 + tid];
-      x0 = c.a0 * zo - c.s0 * vv;
-      zn = c.ks * zo - c.kx * x0;
-      if (c.order == 2) zn -= 0.5f * c.kx * (c.rinv * (x0 - x0_in[b * 64 + tid]));
-      if (step_noise) zn += c.kn * step_noise[((size_t)step * B + b) * 64 + tid];
-    }
-    zs[tid] = zn;
-    if (blockIdx.y == 0) {
-      z_out[b * 64 + tid] = zn;
-      x0_out[b * 64 + tid] = x0;
-      if (latent_out) latent_out[b * 64 + tid] = zn;
-    }
-  }
-  __syncthreads();
-  if (!do_proj) return;
-  const int n = blockIdx.y * 256 + tid;
-  if (n < H) {
-    const uint4* wr = reinterpret_cast<const uint4*>(w_noisy + (size_t)n * 64);
-    float acc = 0.f;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      float wf[8];
-      bf16x8_unpack(wr[c], wf);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc = fmaf(wf[j], zs[c * 8 + j], acc);
-    }
-    xout[(size_t)b * H + n] = acc;
-    xout[(size_t)(B + b) * H + n] = acc;
-  }
-}
+// one DPM-Solver++ step (update formula at SDpm, vv_stream.cuh); kn: per-step noise gain (sde-dpmsolver++), 0 for the ODE solver
+struct DpmCoef { float a0, s0, ks, kx, rinv; int order; float kn; };
 
 // embeds[b] = active[b] ? e_new[b] : embeds[b];  embeds[B+b] = embeds[b]  (negative stream is fed the same input, :579-581)
 __global__ void select_embeds_kernel(float* __restrict__ embeds, const float* __restrict__ e_new, const int* __restrict__ active,

@@ -95,16 +95,8 @@ struct vv_ctx {
   bool finalized = false;
   bool use_graphs = true;
   bool use_pdl = true;
-  bool use_mma_attn = true;
-  bool use_splitk = true;
-  bool fuse_rope = true;
   bf16* s_planes = nullptr; size_t planes_elems = 0;
-  int mma_min_rows = 9;     // M >= this -> tensor-core GEMM (all prologues/epilogues), below -> weight-streaming GEMV (at M = 8 the GEMV streams weights faster)
   int use_wgmma = 1;        // warpgroup (wgmma) GEMM: 0 off, 1 auto (wide GEMMs), 2 every M > 8 GEMM (VV_WGMMA)
-  bool ring_rms = true;     // RMSNorm folded into gemm_mma_ring_kernel (row scale in the epilogue) instead of rows_norm_kernel (VV_NO_RING_RMS=1 -> off)
-  int codec_mma_min_rows = 9;   // codec GEMMs with at least this many rows use the tensor-core ring kernel (VV_CODEC_MMA_MIN_ROWS)
-  bool mma_ring = true;     // 6-stage cp.async ring for both GEMM operands (gemm_mma_ring_kernel); VV_NO_MMA_RING=1 -> old 1-ahead kernel
-  bf16* head_slab = nullptr; size_t head_slab_bytes = 0; size_t l2_persist_bytes = 0; size_t l2_window_max = 0;
   int wr_tasks_min = 296;
   int wr_force = 0;
   int gemv_grid_cap = 0;
@@ -121,7 +113,7 @@ struct vv_ctx {
   // head
   bf16 *h_noisy = nullptr, *h_cond = nullptr, *h_t0 = nullptr, *h_t2 = nullptr, *h_mod = nullptr, *h_final = nullptr;
   std::vector<HeadLayer> head;
-  int n_steps = 0; float* temb = nullptr; DpmCoef* coef_dev = nullptr; float* tfreqs = nullptr;
+  int n_steps = 0; float* temb = nullptr; float* tfreqs = nullptr;
   std::vector<DpmCoef> coef_host; int coef_version = 0;
   bool sde = false; const float* step_noise = nullptr;   // sde-dpmsolver++: per-step variance noise [n_steps][B][64] (vv_set_step_noise)
   // connectors
@@ -136,9 +128,8 @@ struct vv_ctx {
   std::vector<int64_t> kv_len_host; std::vector<std::vector<int>> seq_pages; std::vector<int> free_pages;
   // scratch
   float* s_lgu = nullptr;   // LM gate/up raw sums [2B][2I] (weight-stream path)
-  float *s_h = nullptr, *s_qkv = nullptr, *s_qrot = nullptr, *s_attn = nullptr, *s_act = nullptr, *s_pacc = nullptr, *s_pml = nullptr;
-  int nsplit = 128;
-  float *s_condp = nullptr, *s_call = nullptr, *s_mod = nullptr, *s_hx = nullptr, *s_hg = nullptr, *s_v = nullptr, *s_z = nullptr,
+  float *s_h = nullptr, *s_qkv = nullptr;
+  float *s_condp = nullptr, *s_call = nullptr, *s_mod = nullptr, *s_hx = nullptr, *s_v = nullptr, *s_z = nullptr,
         *s_x0 = nullptr, *s_tfeat = nullptr, *s_t1 = nullptr, *s_hgu = nullptr;
   float *s_xa = nullptr, *s_xb = nullptr, *s_u = nullptr, *s_win = nullptr, *s_xn = nullptr;
   float *s_e = nullptr, *s_c1 = nullptr, *s_feat = nullptr, *s_audio = nullptr, *s_latent = nullptr;
@@ -148,7 +139,6 @@ struct vv_ctx {
   // weight-stream programs (vv_stream.cuh)
   struct StreamProg {
     SOp* ops = nullptr; int n_ops = 0; CUtensorMap* tmaps = nullptr; int n_stages = 0; int b_bytes = 0; int smem = 0; int gemv_ops = 0; int variant = 0;
-    std::vector<int> op_first;           // stage i as built -> its first stage in `ops` (a K-split stage becomes several)
   };
   std::map<std::string, StreamProg> sprogs;
   unsigned* st_bar = nullptr;            // grid-barrier counter of the stream kernel
@@ -156,8 +146,6 @@ struct vv_ctx {
   int st_inflight = 4;                   // VV_STREAM_INFLIGHT: TMA tiles (16 KB) a CTA keeps in flight
   float* dec_front_x = nullptr;                  // where the streamed decoder front leaves its rows (same for every program: fixed structure)
   float *s_cx = nullptr, *s_cu = nullptr;        // codec rows / FFN hidden sums of the stream path (two buffers each)
-  int use_stream = 15;                    // VV_STREAM bit 0: sampler, bit 1: LM linears, bit 2: + LM attention (whole decoder stack as one launch)
-                                         // through the weight-stream kernel; 0 -> kernel-per-stage everywhere
   float* s_rope = nullptr;                        // [2B][64][2] cos / sin of the current positions
   float *s_pacc2 = nullptr, *s_pml2 = nullptr;   // attention partials of the stream path: [2B][kv_heads][SMs][8][128] / [..][8][2]
   std::map<std::tuple<const bf16*, int, int>, bf16*> tiled; size_t tiled_bytes = 0;   // tile-major copies of the weights the stream kernel reads,
@@ -171,10 +159,9 @@ struct vv_ctx {
 
 struct L {  // launcher
   vv_ctx* c; cudaStream_t s;
-  const void* win_base = nullptr;   // optional L2 access-policy window for this launch (persisting hits inside it)
-  size_t win_bytes = 0;
-  float win_ratio = 0.f;
 };
+
+constexpr int MMA_MIN_ROWS = 9;   // M >= this -> tensor-core GEMM (all prologues/epilogues), below -> weight-streaming GEMV (at M = 8 the GEMV streams weights faster)
 
 // every hot-path kernel goes through here: programmatic dependent launch (PDL) lets kernel N+1 be scheduled and run its
 // weight-only prologue while kernel N drains; inside CUDA-graph capture these become programmatic dependency edges.
@@ -183,24 +170,11 @@ static cudaError_t launch_k(const L& l, void (*kern)(KArgs...), dim3 grid, dim3 
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = l.s;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (l.c->use_pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (l.win_bytes) {
-    attr[na].id = cudaLaunchAttributeAccessPolicyWindow;
-    attr[na].val.accessPolicyWindow.base_ptr = const_cast<void*>(l.win_base);
-    attr[na].val.accessPolicyWindow.num_bytes = l.win_bytes;
-    attr[na].val.accessPolicyWindow.hitRatio = l.win_ratio;
-    attr[na].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr[na].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    ++na;
-  }
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = na;
+  cfg.numAttrs = l.c->use_pdl ? 1 : 0;
   l.c->launches++;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
@@ -257,27 +231,25 @@ static int linear(const L& l, GemvP p) {
     CK(launch_k(l, gemm_wgmma_kernel, dim3((p.N + WG_BM - 1) / WG_BM, (p.M + WG_BN - 1) / WG_BN), dim3(128), (size_t)WG_SMEM, p, (const bf16*)hi, (const bf16*)lo));
     return 0;
   }
-  if (p.M >= l.c->mma_min_rows) {
+  if (p.M >= MMA_MIN_ROWS) {
     dim3 grid((p.N + MM_BN - 1) / MM_BN, (p.M + MM_BM - 1) / MM_BM);
     const bool inplace_res = (p.epi == EPI_RESID || p.epi == EPI_GAMMA_RESID || p.epi == EPI_GATED_RESID) && p.res == p.y && p.ldres == p.ldy;
     const int nk = (p.K + MM_BK - 1) / MM_BK;
-    if (l.c->use_splitk && inplace_res && nk >= 8 && (int)(grid.x * grid.y) < l.c->sm_count) {
+    if (inplace_res && nk >= 8 && (int)(grid.x * grid.y) < l.c->sm_count) {
       int z = std::min(std::min(nk / 2, 16), (2 * l.c->sm_count) / (int)(grid.x * grid.y));
       grid.z = std::max(z, 1);
     }
     const bool ring_rms = p.pro == PRO_RMSNORM && grid.z == 1 && p.K <= MR_MAXK_NORM && p.K % 4 == 0;
-    if (l.c->mma_ring && (p.pro == PRO_NONE || ring_rms) && p.epi != EPI_SWIGLU) {
+    if ((p.pro == PRO_NONE || ring_rms) && p.epi != EPI_SWIGLU) {
       // the combinations the codec passes use get their own instantiation (FFN1: folded RMSNorm + GELU; FFN2 / transposed convs: plain or
       // gamma-residual, split-K or not); anything else runs the run-time-switched one
       void (*fn)(GemvP) = gemm_mma_ring_kernel<-1, -1>;
-      if (!getenv("VV_RING_GENERIC")) {
-        if (ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<1, EPI_GELU>;
-        else if (ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<1, EPI_NONE>;
-        else if (!ring_rms && p.epi == EPI_GAMMA_RESID) fn = gemm_mma_ring_kernel<0, EPI_GAMMA_RESID>;
-        else if (!ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<0, EPI_NONE>;
-        else if (!ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<0, EPI_GELU>;
-        else if (!ring_rms && p.epi == EPI_RESID) fn = gemm_mma_ring_kernel<0, EPI_RESID>;
-      }
+      if (ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<1, EPI_GELU>;
+      else if (ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<1, EPI_NONE>;
+      else if (!ring_rms && p.epi == EPI_GAMMA_RESID) fn = gemm_mma_ring_kernel<0, EPI_GAMMA_RESID>;
+      else if (!ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<0, EPI_NONE>;
+      else if (!ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<0, EPI_GELU>;
+      else if (!ring_rms && p.epi == EPI_RESID) fn = gemm_mma_ring_kernel<0, EPI_RESID>;
       CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MR_SMEM_NORM));
       CK(launch_k(l, fn, dim3(grid), dim3(128), (size_t)(ring_rms ? MR_SMEM_NORM : MR_SMEM), p));
       return 0;
@@ -491,12 +463,10 @@ static long long stage_operand_bytes(const vv_ctx* c, const SOp& o, long long KB
 // K split: y += alpha * W pro(x) is a sum over k-blocks and the epilogue is an atomic sum, so a stage whose operand region is too large
 // for the ring runs as consecutive slices over k-block ranges (SP_COMBINE: whole heads).  The first slice keeps the grid barrier, bias,
 // zero-fill jobs and RoPE rows; the others follow without a barrier.  Every slice has its own tile-major weight copy and tensor map.
-// first[i] = index of the first stage that stage i of the builder became (first[n] = stage count).
-static int split_and_map(StreamBuilder& b, long long cap, std::vector<int>* tmap_of, std::vector<int>* first_out) {
+static int split_and_map(StreamBuilder& b, long long cap, std::vector<int>* tmap_of) {
   vv_ctx* c = b.c;
   std::vector<SOp> ops;
-  std::vector<int>& first = *first_out;
-  first.assign(b.ops.size() + 1, 0);
+  std::vector<int> first(b.ops.size() + 1, 0);     // stage i of the builder -> its first stage after the split (first[n] = stage count)
   tmap_of->clear();
   for (size_t i = 0; i < b.ops.size(); ++i) {
     first[i] = (int)ops.size();
@@ -565,7 +535,7 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
   CK(cudaFuncGetAttributes(&fa, STREAM_VARIANTS[pr->variant].fn));
   const int max_dyn = 232448 - (int)fa.sharedSizeBytes - 256;
   std::vector<int> tmap_of;
-  RET(split_and_map(b, b.operand_cap > 0 ? b.operand_cap : (long long)max_dyn - 1024 - (long long)ST_MIN_RING * ST_TILE, &tmap_of, &pr->op_first));
+  RET(split_and_map(b, b.operand_cap > 0 ? b.operand_cap : (long long)max_dyn - 1024 - (long long)ST_MIN_RING * ST_TILE, &tmap_of));
   int b_bytes = 2048;
   for (const SOp& o : b.ops) {
     if (o.kind == SK_MIX && (o.cod.T_out > 8 || o.K % 4 || o.K > 4096)) return fail(VV_ERR_INVALID, "stream: mixer stage handles T <= 8, C <= 4096");
@@ -610,15 +580,8 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
   return 0;
 }
 
-// stages [op_begin, op_begin + op_count) of the program as built (-1: to the end), i.e. with all the slices of K-split stages
-static int launch_stream(const L& l, const vv_ctx::StreamProg& pr, int op_begin = 0, int op_count = -1) {
+static int launch_stream(const L& l, const vv_ctx::StreamProg& pr) {
   vv_ctx* c = l.c;
-  const int n_built = (int)pr.op_first.size() - 1;
-  if (op_count < 0) op_count = n_built - op_begin;
-  if (op_begin < 0 || op_begin + op_count > n_built) return fail(VV_ERR_INVALID, "stream: stages [%d, +%d) outside the program", op_begin, op_count);
-  const int op_end = pr.op_first[op_begin + op_count];
-  op_begin = pr.op_first[op_begin];
-  op_count = op_end - op_begin;
   CK(cudaMemsetAsync(c->st_bar, 0, sizeof(unsigned), l.s));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
@@ -628,10 +591,10 @@ static int launch_stream(const L& l, const vv_ctx::StreamProg& pr, int op_begin 
   attr[0].val.cooperative = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   SParams P;
-  P.ops = pr.ops + op_begin; P.n_ops = op_count; P.bar_count = c->st_bar; P.diag = c->st_diag_dev; P.n_stages = pr.n_stages; P.b_bytes = pr.b_bytes;
+  P.ops = pr.ops; P.n_ops = pr.n_ops; P.bar_count = c->st_bar; P.diag = c->st_diag_dev; P.n_stages = pr.n_stages; P.b_bytes = pr.b_bytes;
   P.max_inflight = std::max(1, std::min(pr.n_stages, c->st_inflight));
   P.kv_len = c->kv_len_dev; P.row_mode = c->row_mode_dev; P.n_seq = 2 * c->d.max_batch; P.kv_heads = c->d.num_kv_heads;
-  P.trace = (c->st_trace && op_count == pr.n_ops && pr.n_ops <= c->st_trace_ops) ? c->st_trace : nullptr; P.trace_cta = c->st_trace_cta;
+  P.trace = (c->st_trace && pr.n_ops <= c->st_trace_ops) ? c->st_trace : nullptr; P.trace_cta = c->st_trace_cta;
   P.trace2 = P.trace ? c->st_trace2 : nullptr;
   if (P.trace) c->st_trace_last_ops = pr.n_ops;
   c->launches++;
@@ -721,23 +684,12 @@ extern "C" int vv_create(const vv_model_desc* desc, int device, vv_ctx** out) {
   c->sm_count = prop.multiProcessorCount;
   const char* ng = getenv("VV_NO_GRAPH");
   c->use_graphs = !(ng && ng[0] == '1');
-  const char* na = getenv("VV_SCALAR_ATTN");
-  c->use_mma_attn = !(na && na[0] == '1');
   c->wr_tasks_min = c->sm_count;      // one task per SM (tools/bench_gemv.py compares geometries)
   if (getenv("VV_WR_TASKS_MIN")) c->wr_tasks_min = atoi(getenv("VV_WR_TASKS_MIN"));
   if (getenv("VV_WR_FORCE")) c->wr_force = atoi(getenv("VV_WR_FORCE"));
   if (getenv("VV_GEMV_GRID_CAP")) c->gemv_grid_cap = atoi(getenv("VV_GEMV_GRID_CAP"));
-  if (getenv("VV_NO_FUSE_ROPE")) c->fuse_rope = false;
-  if (getenv("VV_STREAM")) c->use_stream = atoi(getenv("VV_STREAM"));
   if (getenv("VV_STREAM_INFLIGHT")) c->st_inflight = atoi(getenv("VV_STREAM_INFLIGHT"));
   if (getenv("VV_WGMMA")) c->use_wgmma = atoi(getenv("VV_WGMMA"));
-  if (getenv("VV_MMA_MIN_ROWS")) c->mma_min_rows = atoi(getenv("VV_MMA_MIN_ROWS"));
-  if (getenv("VV_NO_MMA_RING")) c->mma_ring = false;
-  if (getenv("VV_NO_RING_RMS")) c->ring_rms = false;
-  if (getenv("VV_CODEC_MMA_MIN_ROWS")) c->codec_mma_min_rows = atoi(getenv("VV_CODEC_MMA_MIN_ROWS"));
-  else if (getenv("VV_MMA_MIN_ROWS")) c->codec_mma_min_rows = c->mma_min_rows;
-  const char* ns = getenv("VV_NO_SPLITK");
-  c->use_splitk = !(ns && ns[0] == '1');
   const char* np = getenv("VV_NO_PDL");
   c->use_pdl = !(np && np[0] == '1');
   build_expected(c);
@@ -1070,17 +1022,17 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     const size_t modrows = (size_t)(3 * LH + 2) * H;
     RET(dmalloc(c, &c->h_mod, modrows * H, false));
     c->head.resize(LH);
-    // the per-step weights of all head layers live in ONE slab so a single L2 access-policy window can keep (part of) them
-    // resident across the N diffusion steps (they are re-read N times per frame; everything else streams once)
+    // the per-step weights of all head layers live in one slab: per layer interleaved gate/up [2F][H], then down [H][F]
+    // (the sampler program packs its tile-major copies from here)
     const size_t per_layer_el = (size_t)3 * F * H;
-    c->head_slab_bytes = per_layer_el * LH * 2;
-    RET(dmalloc(c, &c->head_slab, per_layer_el * LH, false));
+    bf16* slab;
+    RET(dmalloc(c, &slab, per_layer_el * LH, false));
     for (int l = 0; l < LH; ++l) {
       std::string q = S("%s.layers.%d", h.c_str(), l);
       RawTensor *tg, *tu, *tm, *td;
       RET(need(c, q + ".ffn.gate_proj.weight", &tg, {F, H}));
       RET(need(c, q + ".ffn.up_proj.weight", &tu, {F, H}));
-      c->head[l].wgu = c->head_slab + per_layer_el * l;
+      c->head[l].wgu = slab + per_layer_el * l;
       c->head[l].wdown = c->head[l].wgu + (size_t)2 * F * H;
       interleave_rows_kernel<<<4096, 256>>>((const bf16*)tg->p, (const bf16*)tu->p, c->head[l].wgu, (size_t)F, (size_t)H);
       CKL();
@@ -1097,18 +1049,6 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
       *hb += (int64_t)3 * H * H * 2;
       drop(c, q + ".adaLN_modulation.1.weight");
     }
-    {
-      int maxp = 0, maxw = 0;
-      cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, c->device);
-      cudaDeviceGetAttribute(&maxw, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
-      size_t want = 0;     // off by default (the sampler is latency- rather than bandwidth-bound): opt-in via VV_L2_PERSIST_MB
-      if (getenv("VV_L2_PERSIST_MB")) want = (size_t)atoi(getenv("VV_L2_PERSIST_MB")) << 20;
-      c->l2_persist_bytes = std::min<size_t>(want, (size_t)maxp);
-      c->l2_window_max = (size_t)maxw;
-      if (c->l2_persist_bytes) CK(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, c->l2_persist_bytes));
-      if (getenv("VV_VERBOSE")) fprintf(stderr, "[vv] L2 persisting max %d MB, window max %d MB, using %zu MB for a %zu MB head slab\n", maxp >> 20,
-                                        maxw >> 20, c->l2_persist_bytes >> 20, c->head_slab_bytes >> 20);
-    }
     RawTensor* tm;
     RET(need(c, h + ".final_layer.adaLN_modulation.1.weight", &tm, {2 * H, H}));
     CK(cudaMemcpy(c->h_mod + (size_t)LH * 3 * H * H, tm->p, (size_t)2 * H * H * 2, cudaMemcpyDeviceToDevice));
@@ -1116,7 +1056,6 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     drop(c, h + ".final_layer.adaLN_modulation.1.weight");
     const int NS = std::max(d.max_diffusion_steps, 1);
     RET(dmalloc(c, &c->temb, (size_t)NS * H));
-    RET(dmalloc(c, &c->coef_dev, (size_t)NS));
     RET(dmalloc(c, &c->tfreqs, 128));
     std::vector<float> fr(128);
     for (int j = 0; j < 128; ++j) fr[j] = expf((-9.210340371976184f * (float)j) / 128.0f);
@@ -1139,7 +1078,6 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     memset(c->st_diag_host, 0, 64);
     CK(cudaHostGetDevicePointer((void**)&c->st_diag_dev, c->st_diag_host, 0));
     RET(dmalloc(c, &c->s_hx, (size_t)M2 * H));
-    RET(dmalloc(c, &c->s_hg, (size_t)M2 * F));
     RET(dmalloc(c, &c->s_hgu, (size_t)2 * M2 * 2 * F));
     RET(dmalloc(c, &c->s_v, (size_t)M2 * 64));
     RET(dmalloc(c, &c->s_z, (size_t)2 * B * 64));
@@ -1233,17 +1171,12 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
   // ---------------- LM scratch ----------------
   RET(dmalloc(c, &c->s_h, (size_t)M2 * H));
   RET(dmalloc(c, &c->s_qkv, (size_t)M2 * c->Nqkv));
-  RET(dmalloc(c, &c->s_qrot, (size_t)M2 * nq));
-  RET(dmalloc(c, &c->s_attn, (size_t)M2 * nq));
-  RET(dmalloc(c, &c->s_act, (size_t)M2 * I));
   RET(dmalloc(c, &c->s_lgu, (size_t)M2 * 2 * I));
   RET(dmalloc(c, &c->s_rope, (size_t)M2 * HD));
   RET(dmalloc(c, &c->s_cx, (size_t)2 * B * 8192));
   RET(dmalloc(c, &c->s_cu, (size_t)2 * B * 32768));
   RET(dmalloc(c, &c->s_pacc2, (size_t)M2 * d.num_kv_heads * c->sm_count * 8 * HD));
   RET(dmalloc(c, &c->s_pml2, (size_t)M2 * d.num_kv_heads * c->sm_count * 8 * 2));
-  RET(dmalloc(c, &c->s_pacc, (size_t)M2 * d.num_q_heads * c->nsplit * HD));
-  RET(dmalloc(c, &c->s_pml, (size_t)M2 * d.num_q_heads * c->nsplit * 2));
   RET(dmalloc(c, &c->s_tok, 64));
   RET(dmalloc(c, &c->kv_len_dev, 16));
   RET(dmalloc(c, &c->row_mode_dev, 16));
@@ -1473,48 +1406,9 @@ static int enqueue_lm_head(const L& l, const float* hidden, float* logits, int32
   return 0;
 }
 
-// The linears of decoder layers [li0, li1) as one weight-stream program (vv_stream.cuh), launched in pieces around the attention kernels:
-//   [zero s_qkv | QKV(li0)]  attention(li0)  [O(li0) GU(li0) DN(li0) QKV(li0+1)]  attention(li0+1)  ...  [O GU DN](li1-1)
-// QKV: RMSNorm prologue, bias; O: accumulates into the residual stream; GU: RMSNorm prologue -> raw gate/up sums; DN: SwiGLU prologue,
-// accumulates into the residual stream.  Zero-fill jobs ride on the O stage (s_qkv and the gate/up buffer are dead at that point).
-static int lm_stream_prog(vv_ctx* c, int li0, int li1, const vv_ctx::StreamProg** out) {
-  char key[64];
-  snprintf(key, sizeof key, "lm:%d:%d", li0, li1);
-  auto it = c->sprogs.find(key);
-  if (it != c->sprogs.end()) { *out = &it->second; return 0; }
-  const auto& d = c->d;
-  const int H = d.hidden_size, I = d.intermediate_size, M = 2 * d.max_batch, nq = d.num_q_heads * d.head_dim;
-  StreamBuilder b(c);
-  b.nop(false, c->s_qkv, (long long)M * c->Nqkv);
-  auto qkv = [&](int li) -> int {
-    const LmLayer& y = c->lm[li];
-    SOp* o;
-    RET(b.gemv(y.wqkv, y.bqkv, c->s_h, H, c->s_qkv, c->Nqkv, M, c->Nqkv, H, true, &o));
-    o->pro = SP_RMSNORM; o->pro_w = y.ln1; o->pro_eps = d.rms_norm_eps;
-    return 0;
-  };
-  RET(qkv(li0));
-  for (int li = li0; li < li1; ++li) {
-    const LmLayer& y = c->lm[li];
-    SOp* o;
-    RET(b.gemv(y.wo, nullptr, c->s_attn, nq, c->s_h, H, M, H, nq, false, &o));
-    o->init_dst = c->s_qkv; o->init_n = (long long)M * c->Nqkv;
-    o->init2_dst = c->s_lgu; o->init2_n = (long long)M * 2 * I;
-    RET(b.gemv(y.wgu, nullptr, c->s_h, H, c->s_lgu, 2 * I, M, 2 * I, H, true, &o));
-    o->pro = SP_RMSNORM; o->pro_w = y.ln2; o->pro_eps = d.rms_norm_eps;
-    RET(b.gemv(y.wdown, nullptr, c->s_lgu, 2 * I, c->s_h, H, M, H, I, true, &o));
-    o->pro = SP_SWIGLU;
-    if (li + 1 < li1) RET(qkv(li + 1));
-  }
-  vv_ctx::StreamProg pr;
-  RET(finish_stream(b, &pr));
-  it = c->sprogs.emplace(key, pr).first;
-  *out = &it->second;
-  return 0;
-}
-
-// All of decoder layers [li0, li1) as ONE weight-stream program: per layer QKV -> attention (K/V pages through the ring) -> O (prologue merges
-// the attention partials) -> gate/up -> down.  5 grid barriers per layer, no kernel boundary inside the stack.
+// All of decoder layers [li0, li1) as ONE weight-stream program over the residual stream s_h (rows = 2B sequences; rows with row_mode 0
+// neither read nor append KV): per layer QKV -> attention (K/V pages through the ring) -> O (prologue merges the attention partials) ->
+// gate/up -> down.  5 grid barriers per layer, no kernel boundary inside the stack.
 static int lm_stream_prog_full(vv_ctx* c, int li0, int li1, const vv_ctx::StreamProg** out) {
   char key[64];
   snprintf(key, sizeof key, "lmf:%d:%d", li0, li1);
@@ -1549,54 +1443,6 @@ static int lm_stream_prog_full(vv_ctx* c, int li0, int li1, const vv_ctx::Stream
   return 0;
 }
 
-// decoder layers [li0, li1) over the residual stream s_h (rows = 2B sequences; rows with row_mode 0 neither read nor append KV)
-static int enqueue_lm_layers(const L& l, int li0, int li1, const vv_ctx::StreamProg* sprog = nullptr) {
-  vv_ctx* c = l.c;
-  const auto& d = c->d;
-  const int H = d.hidden_size, I = d.intermediate_size, M = 2 * d.max_batch, nq = d.num_q_heads * HD;
-  const size_t per_layer = (size_t)c->n_pages * d.num_kv_heads * KV_PAGE * HD;
-  const float scale = 1.0f / sqrtf((float)HD);
-  if (sprog && (c->use_stream & 4)) return launch_stream(l, *sprog);      // whole stack, attention included
-  if (d.head_dim != HD) return fail(VV_ERR_INVALID, "head_dim %d runs through the weight-stream path only (VV_STREAM bit 2)", d.head_dim);
-  if (sprog) RET(launch_stream(l, *sprog, 0, 2));
-  for (int li = li0; li < li1; ++li) {
-    const LmLayer& y = c->lm[li];
-    GemvP p = mk(y.wqkv, y.bqkv, c->s_h, H, c->s_qkv, c->Nqkv, M, c->Nqkv, H);
-    p.pro = PRO_RMSNORM; p.pro_w = y.ln1; p.pro_eps = d.rms_norm_eps;
-    if (!sprog) RET(linear(l, p));
-    KvView kv;
-    kv.kpool = c->kpool + per_layer * li; kv.vpool = c->vpool + per_layer * li;
-    kv.page_table = c->page_table_dev; kv.max_pages = c->max_pages; kv.kv_len = c->kv_len_dev; kv.row_mode = c->row_mode_dev;
-    kv.kv_heads = d.num_kv_heads; kv.q_heads = d.num_q_heads;
-    if (c->use_mma_attn && c->fuse_rope) {
-      CK(cudaFuncSetAttribute(attn_partial_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AT2_SMEM));
-      CK(launch_k(l, attn_partial_mma_kernel, dim3(c->nsplit, d.num_kv_heads, M), dim3(128), (size_t)AT2_SMEM, c->s_qkv, 1, c->inv_freq, kv, c->s_pacc,
-                  c->s_pml, c->nsplit, scale));
-    } else {
-      CK(launch_k(l, rope_append_kernel, dim3(M), dim3(256), 0, c->s_qkv, c->s_qrot, kv, c->inv_freq));
-      if (c->use_mma_attn) {
-        CK(cudaFuncSetAttribute(attn_partial_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AT2_SMEM));
-        CK(launch_k(l, attn_partial_mma_kernel, dim3(c->nsplit, d.num_kv_heads, M), dim3(128), (size_t)AT2_SMEM, c->s_qrot, 0, c->inv_freq, kv, c->s_pacc,
-                    c->s_pml, c->nsplit, scale));
-      } else {
-        CK(launch_k(l, attn_partial_kernel, dim3(c->nsplit, d.num_kv_heads, M), dim3(128), 0, c->s_qrot, kv, c->s_pacc, c->s_pml, c->nsplit, scale));
-      }
-    }
-    CK(launch_k(l, attn_combine_kernel, dim3(d.num_q_heads, M), dim3(128), 0, c->s_pacc, c->s_pml, c->row_mode_dev, c->s_attn, d.num_q_heads, c->nsplit));
-    if (sprog) { RET(launch_stream(l, *sprog, 2 + 4 * (li - li0), li + 1 < li1 ? 4 : 3)); continue; }
-    p = mk(y.wo, nullptr, c->s_attn, nq, c->s_h, H, M, H, nq);
-    p.epi = EPI_RESID; p.res = c->s_h; p.ldres = H;
-    RET(linear(l, p));
-    p = mk(y.wgu, nullptr, c->s_h, H, c->s_act, I, M, 2 * I, H);
-    p.pro = PRO_RMSNORM; p.pro_w = y.ln2; p.pro_eps = d.rms_norm_eps; p.epi = EPI_SWIGLU;
-    RET(linear(l, p));
-    p = mk(y.wdown, nullptr, c->s_act, I, c->s_h, H, M, H, I);
-    p.epi = EPI_RESID; p.res = c->s_h; p.ldres = H;
-    RET(linear(l, p));
-  }
-  return 0;
-}
-
 static int enqueue_final_norm(const L& l, float* hidden) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
@@ -1606,11 +1452,11 @@ static int enqueue_final_norm(const L& l, float* hidden) {
   return 0;
 }
 
-static int enqueue_lm_decode(const L& l, const float* embeds, float* hidden, float* logits, int32_t* tokens, const vv_ctx::StreamProg* sprog) {
+static int enqueue_lm_decode(const L& l, const float* embeds, float* hidden, float* logits, int32_t* tokens, const vv_ctx::StreamProg& sprog) {
   vv_ctx* c = l.c;
   const int H = c->d.hidden_size, M = 2 * c->d.max_batch;
   CK(cudaMemcpyAsync(c->s_h, embeds, (size_t)M * H * 4, cudaMemcpyDeviceToDevice, l.s));
-  RET(enqueue_lm_layers(l, 0, c->d.num_layers, sprog));
+  RET(launch_stream(l, sprog));
   RET(enqueue_final_norm(l, hidden));
   return enqueue_lm_head(l, hidden, logits, tokens);
 }
@@ -1619,11 +1465,11 @@ static int enqueue_lm_decode(const L& l, const float* embeds, float* hidden, flo
 // (modeling_vibevoice_streaming.py:134-146); each stack keeps its own KV sequences (lengths differ: the upper stack also sees the speech
 // positions).  One call runs layers [begin, end) for the rows enabled by vv_set_row_mode, appends their K/V speculatively at kv_len (commit
 // with vv_kv_commit as for vv_lm_decode) and returns the residual stream -- normalised with the model's final norm iff final_norm != 0.
-static int enqueue_lm_range(const L& l, const float* embeds, int li0, int li1, int final_norm, float* hidden, const vv_ctx::StreamProg* sprog) {
+static int enqueue_lm_range(const L& l, const float* embeds, int final_norm, float* hidden, const vv_ctx::StreamProg& sprog) {
   vv_ctx* c = l.c;
   const int H = c->d.hidden_size, M = 2 * c->d.max_batch;
   CK(cudaMemcpyAsync(c->s_h, embeds, (size_t)M * H * 4, cudaMemcpyDeviceToDevice, l.s));
-  RET(enqueue_lm_layers(l, li0, li1, sprog));
+  RET(launch_stream(l, sprog));
   if (final_norm) return enqueue_final_norm(l, hidden);
   CK(cudaMemcpyAsync(hidden, c->s_h, (size_t)M * H * 4, cudaMemcpyDeviceToDevice, l.s));
   return 0;
@@ -1635,10 +1481,9 @@ extern "C" int vv_lm_decode(vv_ctx* c, const float* embeds, float* hidden, float
   for (int s = 0; s < 2 * c->d.max_batch; ++s) RET(vv_kv_reserve(c, s, c->kv_len_host[s] + 1, stream));
   char key[256];
   snprintf(key, sizeof key, "lm:%p:%p:%p:%p", (const void*)embeds, (void*)hidden, (void*)logits, (void*)tokens);
-  const vv_ctx::StreamProg* sprog = nullptr;      // built outside stream capture
-  if (c->use_stream & 4) RET(lm_stream_prog_full(c, 0, c->d.num_layers, &sprog));
-  else if (c->use_stream & 2) RET(lm_stream_prog(c, 0, c->d.num_layers, &sprog));
-  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_lm_decode(l, embeds, hidden, logits, tokens, sprog); });
+  const vv_ctx::StreamProg* sprog;      // built outside stream capture
+  RET(lm_stream_prog_full(c, 0, c->d.num_layers, &sprog));
+  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_lm_decode(l, embeds, hidden, logits, tokens, *sprog); });
 }
 extern "C" int vv_lm_head(vv_ctx* c, const float* hidden, float* logits, int32_t* tokens, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
@@ -1667,10 +1512,9 @@ extern "C" int vv_lm_decode_range(vv_ctx* c, const float* embeds, int layer_begi
   for (int s = 0; s < 2 * c->d.max_batch; ++s) RET(vv_kv_reserve(c, s, c->kv_len_host[s] + 1, stream));
   char key[256];
   snprintf(key, sizeof key, "lmr:%p:%p:%d:%d:%d", (const void*)embeds, (void*)hidden, layer_begin, layer_end, final_norm);
-  const vv_ctx::StreamProg* sprog = nullptr;
-  if (c->use_stream & 4) RET(lm_stream_prog_full(c, layer_begin, layer_end, &sprog));
-  else if (c->use_stream & 2) RET(lm_stream_prog(c, layer_begin, layer_end, &sprog));
-  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_lm_range(l, embeds, layer_begin, layer_end, final_norm, hidden, sprog); });
+  const vv_ctx::StreamProg* sprog;
+  RET(lm_stream_prog_full(c, layer_begin, layer_end, &sprog));
+  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_lm_range(l, embeds, final_norm, hidden, *sprog); });
 }
 
 extern "C" int vv_embed_tokens(vv_ctx* c, const int32_t* tokens_host, int n, float* out, void* stream) {
@@ -1720,7 +1564,6 @@ static int set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, c
   c->coef_host = cf;
   c->coef_version++;
   CK(cudaStreamSynchronize(s));
-  CK(cudaMemcpy(c->coef_dev, cf.data(), sizeof(DpmCoef) * n_steps, cudaMemcpyHostToDevice));
   float* tdev = c->s_t1;   // reuse as staging for the timesteps (n floats) before it is overwritten below
   CK(cudaMemcpy(tdev, timesteps, sizeof(float) * n_steps, cudaMemcpyHostToDevice));
   timestep_feat_kernel<<<n_steps, 256, 0, s>>>(tdev, c->tfreqs, c->s_tfeat, n_steps);
@@ -1739,28 +1582,6 @@ static int set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, c
   return 0;
 }
 
-// head ops of one diffusion step (shared by the kernel-per-stage path and the program builder)
-static void head_step_gemvs(vv_ctx* c, int i, std::vector<GemvP>* out) {
-  const auto& d = c->d;
-  const int H = d.hidden_size, F = d.head_ffn_dim, M = 2 * d.max_batch, LH = d.head_layers;
-  const int modld = (3 * LH + 2) * H;
-  const float* mod = c->s_mod + (size_t)i * M * modld;
-  for (int li = 0; li < LH; ++li) {
-    const HeadLayer& hl = c->head[li];
-    GemvP p = mk(hl.wgu, nullptr, c->s_hx, H, c->s_hg, F, M, 2 * F, H);
-    p.pro = PRO_ADALN; p.pro_w = hl.norm; p.pro_eps = d.head_rms_eps;
-    p.pro_shift = mod + (size_t)li * 3 * H; p.pro_scale = mod + (size_t)li * 3 * H + H; p.pro_ld = modld;
-    p.epi = EPI_SWIGLU;
-    out->push_back(p);
-    p = mk(hl.wdown, nullptr, c->s_hg, F, c->s_hx, H, M, H, F);
-    p.epi = EPI_GATED_RESID; p.epi_a = mod + (size_t)li * 3 * H + 2 * H; p.epi_lda = modld; p.res = c->s_hx; p.ldres = H;
-    out->push_back(p);
-  }
-  GemvP p = mk(c->h_final, nullptr, c->s_hx, H, c->s_v, 64, M, 64, H);
-  p.pro = PRO_ADALN; p.pro_w = nullptr; p.pro_eps = d.head_rms_eps;
-  p.pro_shift = mod + (size_t)LH * 3 * H; p.pro_scale = mod + (size_t)LH * 3 * H + H; p.pro_ld = modld;
-  out->push_back(p);
-}
 __global__ void set_float_kernel(float* p, float v) { *p = v; }
 // the CFG scale is read from device memory by the solver kernels, so one captured graph serves every value (a service with a
 // user-controlled cfg_scale would otherwise capture and keep one frame-tail graph per distinct float)
@@ -1834,10 +1655,10 @@ static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out,
   return 0;
 }
 
-static int enqueue_diffusion(const L& l, const float* cond, const float* noise, float* latent_out, const vv_ctx::StreamProg* sprog) {
+static int enqueue_diffusion(const L& l, const float* cond, const vv_ctx::StreamProg& sprog) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
-  const int H = d.hidden_size, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = c->n_steps;
+  const int H = d.hidden_size, M = 2 * d.max_batch, LH = d.head_layers, N = c->n_steps;
   if (N < 1) return fail(VV_ERR_STATE, "vv_set_diffusion_steps not called");
   const int modld = (3 * LH + 2) * H;
   if (c->sde && !c->step_noise) return fail(VV_ERR_STATE, "sde-dpmsolver++ needs vv_set_step_noise before sampling");
@@ -1851,27 +1672,7 @@ static int enqueue_diffusion(const L& l, const float* cond, const float* noise, 
   // (the reference recomputes Linear(silu(c)) inside every head call, diffusion_head.py:159, 185; c depends only on (cond, t_i))
   p = mk(c->h_mod, nullptr, c->s_call, H, c->s_mod, modld, N * M, modld, H);
   RET(linear(l, p));
-  if (sprog) return launch_stream(l, *sprog);
-  CK(launch_k(l, dpm_update_proj_kernel, dim3(B, (H + 255) / 256), dim3(256), 0, c->s_z + B * 64, c->s_z, c->s_x0 + B * 64, c->s_x0, c->s_v, noise,
-              c->coef_dev, -1, (const float*)c->cfg_dev, c->h_noisy, c->s_hx, nullptr, B, H, 1, (const float*)nullptr));
-  L lh = l;
-  if (c->l2_persist_bytes && c->head_slab_bytes) {
-    lh.win_base = c->head_slab;
-    lh.win_bytes = std::min(c->head_slab_bytes, c->l2_window_max);
-    lh.win_ratio = std::min(1.0f, (float)c->l2_persist_bytes / (float)lh.win_bytes);
-  }
-  for (int i = 0; i < N; ++i) {
-    std::vector<GemvP> g;
-    head_step_gemvs(c, i, &g);
-    for (auto& q : g) RET(linear(lh, q));
-    const bool last = (i == N - 1);
-    const float* z_in = c->s_z + (size_t)(i & 1) * B * 64; float* z_out = c->s_z + (size_t)((i + 1) & 1) * B * 64;
-    const float* x0_in = c->s_x0 + (size_t)(i & 1) * B * 64; float* x0_out = c->s_x0 + (size_t)((i + 1) & 1) * B * 64;
-    CK(launch_k(l, dpm_update_proj_kernel, dim3(B, last ? 1 : (H + 255) / 256), dim3(256), 0, z_in, z_out, x0_in, x0_out, (const float*)c->s_v, noise,
-                (const DpmCoef*)c->coef_dev, i, (const float*)c->cfg_dev, (const bf16*)c->h_noisy, c->s_hx, last ? latent_out : (float*)nullptr, B, H,
-                last ? 0 : 1, c->sde ? c->step_noise : (const float*)nullptr));
-  }
-  return 0;
+  return launch_stream(l, sprog);
 }
 
 extern "C" int vv_diffusion_sample(vv_ctx* c, const float* cond, const float* noise, const int32_t* active, float cfg, float* latent_out,
@@ -1882,9 +1683,9 @@ extern "C" int vv_diffusion_sample(vv_ctx* c, const float* cond, const float* no
   RET(set_cfg(c, cfg, (cudaStream_t)stream));
   char key[256];
   snprintf(key, sizeof key, "diff:%p:%p:%p", (const void*)cond, (const void*)noise, (void*)latent_out);
-  const vv_ctx::StreamProg* sprog = nullptr;      // built outside stream capture (it allocates and copies)
-  if (c->use_stream & 1) RET(sampler_stream_prog(c, noise, latent_out, &sprog));
-  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_diffusion(l, cond, noise, latent_out, sprog); });
+  const vv_ctx::StreamProg* sprog;      // built outside stream capture (it allocates and copies)
+  RET(sampler_stream_prog(c, noise, latent_out, &sprog));
+  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_diffusion(l, cond, *sprog); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1908,7 +1709,7 @@ static int enqueue_block(const L& l, const Block& b, const float* xin, float* xo
     CK(launch_k(l, dwconv_res_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, xin, c->s_win, b.dw_w, b.dw_b, b.gamma, xout, B, T, C));
   }
   GemvP p;
-  if (M < c->mma_min_rows || (c->ring_rms && c->mma_ring && C <= MR_MAXK_NORM && c->use_wgmma != 2)) {
+  if (M < MMA_MIN_ROWS || (C <= MR_MAXK_NORM && c->use_wgmma != 2)) {
     p = mk(b.w1, b.b1, xout, C, c->s_u, 4 * C, M, 4 * C, C);
     p.pro = PRO_RMSNORM; p.pro_w = b.ffn_norm_w; p.pro_eps = eps; p.epi = EPI_GELU;
     RET(linear(l, p));
@@ -1939,12 +1740,6 @@ static int conv_apply(const L& l, const ConvL& cv, const float* win, float* y, i
   return linear(l, p);
 }
 
-struct ScopedMinRows {     // the codec stages may use a different GEMV/GEMM row threshold than the LM and the sampler
-  vv_ctx* c; int saved;
-  ScopedMinRows(vv_ctx* c_, int v) : c(c_), saved(c_->mma_min_rows) { c->mma_min_rows = v; }
-  ~ScopedMinRows() { c->mma_min_rows = saved; }
-};
-
 // ---- codec stages with B*T <= 8 rows (96 % of the codec's weights: 2048- and 1024-wide blocks, stem / up- / down-sampling convolutions
 // next to them) as weight-stream programs (vv_stream.cuh: SP_WINDOW, SP_MIXER): two stages per Block1D instead of five kernels ------------
 // Buffers: rows ping-pong between X[0] / X[1], FFN hidden sums between U[0] / U[1].  A block reads X[a], its owner CTA stores x1 into X[a^1]
@@ -1952,7 +1747,7 @@ struct ScopedMinRows {     // the codec stages may use a different GEMV/GEMM row
 // buffer's last reader.
 static bool codec_stream_stage(const vv_ctx* c, const Codec& k, int i) {
   const long long rows = (long long)c->d.max_batch * k.T[i];
-  return (c->use_stream & 8) && k.T[i] <= 8 && rows <= 32;
+  return k.T[i] <= 8 && rows <= 32;
 }
 static long long codec_x_floats(const vv_ctx* c) { return (long long)c->d.max_batch * 8192; }
 static long long codec_u_floats(const vv_ctx* c) { return (long long)c->d.max_batch * 32768; }
@@ -1998,15 +1793,15 @@ static int stage_ops(StreamBuilder& b, vv_ctx* c, CodecBufs& cb, const std::vect
   return 0;
 }
 
-// decoder front: stem conv + the leading stages with <= 8 rows; *n_front = stages covered, *out_x = where the last one leaves its rows
+// decoder front: stem conv + the leading stages with <= 8 rows; *n_front = stages covered (at least stage 0: T = 1, B <= 8 rows), *out_x =
+// where the last one leaves its rows
 static int dec_front_prog(vv_ctx* c, const float* latent, const vv_ctx::StreamProg** out, int* n_front, float** out_x) {
   Codec& k = c->dec;
   const auto& d = c->d;
   const int B = d.max_batch;
-  int nf = 0;
+  int nf = 1;
   while (nf < d.n_stages - 1 && codec_stream_stage(c, k, nf)) ++nf;
-  *n_front = nf; *out = nullptr; *out_x = nullptr;
-  if (nf == 0) return 0;
+  *n_front = nf;
   char key[96];
   snprintf(key, sizeof key, "decf:%p", (const void*)latent);
   {
@@ -2041,11 +1836,11 @@ static int dec_front_prog(vv_ctx* c, const float* latent, const vv_ctx::StreamPr
   return 0;
 }
 
-// encoder back: the trailing stages with <= 8 rows, each behind its strided conv, + the head conv.  `xin` = rows entering the conv of the
-// first covered stage (produced by the kernel-per-stage path).
+// encoder back: the trailing stages with <= 8 rows (at least the last one: T = 1, B <= 8 rows), each behind its strided conv, + the head
+// conv.  `xin` = rows entering the conv of the first covered stage (produced by the kernel-per-stage path).
 static int enc_back_first(const vv_ctx* c) {
   const Codec& k = c->enc;
-  int f = c->d.n_stages;
+  int f = c->d.n_stages - 1;
   while (f > 1 && codec_stream_stage(c, k, f - 1)) --f;
   return f;
 }
@@ -2053,8 +1848,6 @@ static int enc_back_prog(vv_ctx* c, const float* xin, float* feat, const vv_ctx:
   Codec& k = c->enc;
   const auto& d = c->d;
   const int B = d.max_batch, ns = d.n_stages, f = enc_back_first(c);
-  *out = nullptr;
-  if (f >= ns) return 0;
   char key[96];
   snprintf(key, sizeof key, "encb:%p:%p", (const void*)xin, (void*)feat);
   auto it = c->sprogs.find(key);
@@ -2084,35 +1877,23 @@ static int enc_back_prog(vv_ctx* c, const float* xin, float* feat, const vv_ctx:
   return 0;
 }
 
-static int enqueue_decode(const L& l, const float* latent, const int32_t* active, float* audio, const vv_ctx::StreamProg* front = nullptr,
-                          int n_front = 0, float* front_x = nullptr) {
+static int enqueue_decode(const L& l, const int32_t* active, float* audio, const vv_ctx::StreamProg& front, int n_front, float* front_x) {
   vv_ctx* c = l.c;
-  ScopedMinRows scoped(c, c->codec_mma_min_rows);
   const auto& d = c->d;
   Codec& k = c->dec;
   const int B = d.max_batch, ns = d.n_stages;
-  float *xa = c->s_xa, *xb = c->s_xb;
-  if (front) {
-    RET(launch_stream(l, *front));              // stem + stages [0, n_front) through the weight-stream kernel
-    xa = front_x;
-  } else {
-    n_front = 0;
-    // stem: window over the last 7 (un-scaled) latent frames; un-scaling latent/scale - bias (:636) is folded in
-    RET(assemble(l, latent, k.convs[0].hist, c->s_win, k.convs[0].next, B, 1, 6, 64, nullptr, 0.f, 1.0f / c->speech_scale, -c->speech_bias));
-    RET(conv_apply(l, k.convs[0], c->s_win, xa, B, 1, 1));
-  }
-  for (int i = n_front; i < ns; ++i) {
-    if (i > 0) {
-      const ConvL& cv = k.convs[i];
-      const int Tin = k.T[i - 1];
-      RET(assemble(l, xa, cv.hist, c->s_win, cv.next, B, Tin, 1, cv.Cin, nullptr, 0.f, 1.f, 0.f));
-      RowMap xm; xm.T = Tin; xm.bs = (long long)(1 + Tin) * cv.Cin; xm.rs = cv.Cin;
-      float* dst = (xa == c->s_xa) ? c->s_xb : c->s_xa;
-      GemvP p = mk(cv.w, cv.bias, c->s_win, 0, dst, cv.N, B * Tin, cv.N, cv.K);
-      p.xmap = xm;
-      RET(linear(l, p));
-      xa = dst; xb = (xa == c->s_xa) ? c->s_xb : c->s_xa;
-    }
+  RET(launch_stream(l, front));                 // stem + stages [0, n_front) through the weight-stream kernel
+  float *xa = front_x, *xb = c->s_xb;
+  for (int i = n_front; i < ns; ++i) {          // i >= 1: every remaining stage starts with its transposed conv
+    const ConvL& cv = k.convs[i];
+    const int Tin = k.T[i - 1];
+    RET(assemble(l, xa, cv.hist, c->s_win, cv.next, B, Tin, 1, cv.Cin, nullptr, 0.f, 1.f, 0.f));
+    RowMap xm; xm.T = Tin; xm.bs = (long long)(1 + Tin) * cv.Cin; xm.rs = cv.Cin;
+    float* dst = (xa == c->s_xa) ? c->s_xb : c->s_xa;
+    GemvP p = mk(cv.w, cv.bias, c->s_win, 0, dst, cv.N, B * Tin, cv.N, cv.K);
+    p.xmap = xm;
+    RET(linear(l, p));
+    xa = dst; xb = (xa == c->s_xa) ? c->s_xb : c->s_xa;
     for (const Block& b : k.stages[i]) { RET(enqueue_block(l, b, xa, xb, B, k.T[i], d.codec_eps)); std::swap(xa, xb); }
   }
   const ConvL& hd = k.convs[ns];
@@ -2135,13 +1916,12 @@ static float* encode_front_out(vv_ctx* c, int first) {
   }
   return in_a ? c->s_xa : c->s_xb;
 }
-static int enqueue_encode(const L& l, const float* audio, const int32_t* active, float* feat, const vv_ctx::StreamProg* back = nullptr) {
+static int enqueue_encode(const L& l, const float* audio, const int32_t* active, const vv_ctx::StreamProg& back) {
   vv_ctx* c = l.c;
-  ScopedMinRows scoped(c, c->codec_mma_min_rows);
   const auto& d = c->d;
   Codec& k = c->enc;
-  const int B = d.max_batch, ns = d.n_stages;
-  const int stop = back ? enc_back_first(c) : ns;
+  const int B = d.max_batch;
+  const int stop = enc_back_first(c);
   float *xa = c->s_xa, *xb = c->s_xb;
   int hop = k.T[0];
   RET(assemble(l, audio, k.convs[0].hist, c->s_win, k.convs[0].next, B, hop, 6, 1, nullptr, 0.f, 1.f, 0.f));
@@ -2156,14 +1936,8 @@ static int enqueue_encode(const L& l, const float* audio, const int32_t* active,
     }
     for (const Block& b : k.stages[i]) { RET(enqueue_block(l, b, xa, xb, B, k.T[i], d.codec_eps)); std::swap(xa, xb); }
   }
-  if (back) {
-    if (xa != encode_front_out(c, stop)) return fail(VV_ERR_STATE, "encoder hand-off buffer mismatch");
-    RET(launch_stream(l, *back));
-  } else {
-    const ConvL& hd = k.convs[ns];
-    RET(assemble(l, xa, hd.hist, c->s_win, hd.next, B, 1, 6, hd.Cin, nullptr, 0.f, 1.f, 0.f));
-    RET(conv_apply(l, hd, c->s_win, feat, B, 1, 1));
-  }
+  if (xa != encode_front_out(c, stop)) return fail(VV_ERR_STATE, "encoder hand-off buffer mismatch");
+  RET(launch_stream(l, back));                  // stages [stop, ns) + head conv through the weight-stream kernel
   CK(launch_k(l, advance_kernel, dim3(k.n_segs, B, ADV_SLICES), dim3(256), 0, k.segs_dev, active));
   return 0;
 }
@@ -2191,18 +1965,18 @@ extern "C" int vv_codec_decode_frame(vv_ctx* c, const float* latent, const int32
   CK(cudaSetDevice(c->device));
   char key[256];
   snprintf(key, sizeof key, "dec:%p:%p:%p", (const void*)latent, (const void*)active, (void*)audio_out);
-  const vv_ctx::StreamProg* front = nullptr; int nf = 0; float* fx = nullptr;
+  const vv_ctx::StreamProg* front; int nf; float* fx;
   RET(dec_front_prog(c, latent, &front, &nf, &fx));
-  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_decode(l, latent, active, audio_out, front, nf, fx); });
+  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_decode(l, active, audio_out, *front, nf, fx); });
 }
 extern "C" int vv_semantic_encode_frame(vv_ctx* c, const float* audio, const int32_t* active, float* feat_out, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
   CK(cudaSetDevice(c->device));
   char key[256];
   snprintf(key, sizeof key, "enc:%p:%p:%p", (const void*)audio, (const void*)active, (void*)feat_out);
-  const vv_ctx::StreamProg* back = nullptr;
+  const vv_ctx::StreamProg* back;
   RET(enc_back_prog(c, encode_front_out(c, enc_back_first(c)), feat_out, &back));
-  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_encode(l, audio, active, feat_out, back); });
+  return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_encode(l, audio, active, *back); });
 }
 extern "C" int vv_connect(vv_ctx* c, const float* latent, const float* sem, const int32_t* active, float* embeds, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
@@ -2218,15 +1992,14 @@ extern "C" int vv_frame_tail(vv_ctx* c, const float* hidden, const float* noise,
   RET(set_cfg(c, cfg, (cudaStream_t)stream));
   snprintf(key, sizeof key, "tail:%p:%p:%p:%p:%p:%p", (const void*)hidden, (const void*)noise, (const void*)active, (void*)latent_out,
            (void*)audio_out, (void*)embeds);
-  const vv_ctx::StreamProg* sprog = nullptr;
-  if (c->use_stream & 1) RET(sampler_stream_prog(c, noise, latent_out, &sprog));
-  const vv_ctx::StreamProg *front = nullptr, *back = nullptr; int nf = 0; float* fx = nullptr;
+  const vv_ctx::StreamProg *sprog, *front, *back; int nf; float* fx;
+  RET(sampler_stream_prog(c, noise, latent_out, &sprog));
   RET(dec_front_prog(c, latent_out, &front, &nf, &fx));
   RET(enc_back_prog(c, encode_front_out(c, enc_back_first(c)), c->s_feat, &back));
   return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) {
-    RET(enqueue_diffusion(l, hidden, noise, latent_out, sprog));
-    RET(enqueue_decode(l, latent_out, active, audio_out, front, nf, fx));
-    RET(enqueue_encode(l, audio_out, active, c->s_feat, back));
+    RET(enqueue_diffusion(l, hidden, *sprog));
+    RET(enqueue_decode(l, active, audio_out, *front, nf, fx));
+    RET(enqueue_encode(l, audio_out, active, *back));
     return enqueue_connect(l, latent_out, c->s_feat, active, embeds);
   });
 }

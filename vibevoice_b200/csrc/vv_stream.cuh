@@ -32,7 +32,8 @@
 // height where a program allows it, descriptor fields in registers, descriptor-only arithmetic between barrier arrival and barrier wait, and
 // uniform early exits instead of predicated-off rows.
 //
-// Reference arithmetic: the stages are the same linears as the stand-alone kernels in vv_kernels.cuh (see the anchors there).
+// Reference arithmetic: the linear stages are the same linears as the stand-alone kernels in vv_kernels.cuh (see the anchors there);
+// attention and the solver update cite theirs at SAtt and SDpm.
 #pragma once
 #include "vv_kernels.cuh"
 
@@ -101,8 +102,12 @@ enum SKind { SK_GEMV = 0, SK_NOP = 1, SK_ATTN = 2, SK_MIX = 3 };
 enum SPro { SP_NONE = 0, SP_RMSNORM = 1, SP_ADALN = 2, SP_SWIGLU = 3, SP_GELU = 4, SP_DPM = 5, SP_SILU = 6, SP_COMBINE = 7, SP_WINDOW = 8, SP_MIXER = 9 };
 enum SAlpha { SA_ONE = 0, SA_GATE = 1 /* alpha[m][n], row stride lda */, SA_GAMMA = 2 /* alpha[n] */ };
 
-// CFG + DPM-Solver++ update of step `step` (same arithmetic as dpm_update_proj_kernel), evaluated in the prologue of the stage that
-// projects the new latent (noisy_images_proj): B-operand row m = z'[m mod B].
+// CFG + DPM-Solver++(2M) update of step `step`, evaluated in the prologue of the stage that projects the new latent (noisy_images_proj):
+// B-operand row m = z'[m mod B].  Rows b (conditional) and B+b (unconditional) of the head output v give
+//   v = v_u + s (v_c - v_u); x0 = a0 z - s0 v; z' = ks z - kx x0 [- 0.5 kx rinv (x0 - x0_prev)] [+ kn * step_noise[step]]
+// (modeling_vibevoice_inference.py:703-709 + schedule/dpm_solver.py:581-584, 669-677, 738-764; sde-dpmsolver++, dpm_solver.py:680-686 /
+// 785-793: same two forms with other ks / kx plus the variance-noise term; step_noise is [n_steps][B][64] or nullptr for the ODE solver).
+// step = -1: z' = the initial noise.
 struct SDpm {
   const float* z_in; float* z_out; const float* x0_in; float* x0_out; const float* v; const float* noise;
   const float* cfg_p; const float* step_noise; float* latent_out;
@@ -116,6 +121,7 @@ struct SDpm {
 // SWIZZLE_128B), so the KV cache streams through the same ring, prefetched across the grid barriers like the weights.
 // A CTA's run of units inside one (m, g) is a segment: one online-softmax partial (max, sum, acc[G heads][128]) written to slot
 // `cta - first_cta(m, g)` of part_acc / part_ml; SP_COMBINE merges the partials of a head while it stages the o-projection's activations.
+// Reference: transformers Qwen2Attention (modeling_qwen2.py:116-174).
 struct SAtt {
   const float* qkv;            // [M][(q_heads + 2 kv_heads) * 128] fp32, bias added, not rotated
   KvView kv;                   // this layer's pool pointers (new K/V rows are written here), page table, kv_len, row_mode
@@ -1113,7 +1119,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
           }
         }
       } else if (PRO_IS(SP_DPM)) {
-        // z' for every sample (same arithmetic as dpm_update_proj_kernel); every CTA with work recomputes it, the owner of unit 0 publishes
+        // z' for every sample (formula at SDpm); every CTA with work recomputes it, the owner of unit 0 publishes
         const SDpm& d = op.dpm;
         for (int i = wt; i < d.B * 64; i += ST_WORKERS) {
           const int b = i >> 6, e = i & 63;
