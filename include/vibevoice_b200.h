@@ -193,6 +193,28 @@ int vv_debug_kv_read(vv_ctx* ctx, int seq, int layer, int64_t pos0, int64_t n, v
 int64_t vv_launch_count(vv_ctx* ctx);     /* kernels launched by this ctx so far */
 int vv_debug_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, float* y, int M, int N, int K,
                   int prologue, const float* pro_w, float eps, int epilogue, void* stream);
+/* the same dispatch (GEMV, tensor-core GEMMs, wgmma) with every feature the codec passes use: y[m][n] = epi(W pro(x_m) + bias[n]).
+ * Row m = (b, t) = (m / map_T, m % map_T) of x starts at x + b * map_bs + t * ldx floats (map_T = 0: dense rows ldx apart); rows may
+ * overlap, which is how a convolution reads its window.  prologue: 0 none, 1 RMSNorm(pro_w, eps), 3 SiLU.  epilogue: 0 none, 2 + res,
+ * 3 res + epi_a[m][n] (rows epi_lda apart) *, 4 res + epi_a[n] *, 6 GELU, 7 SiLU; res rows ldres apart; res == y with ldres == ldy runs
+ * in place, and on grids smaller than the GPU the tensor-core GEMMs then split K and add into y with fp32 atomics.  info[2] = {kernel,
+ * split-K factor}: kernel 0 GEMV, 1..7 gemm_mma_ring_kernel <1,GELU> <1,NONE> <0,GAMMA_RESID> <0,NONE> <0,GELU> <0,RESID> <-1,-1>,
+ * 8 gemm_mma_kernel, 9 split_bf16_kernel + gemm_wgmma_kernel.  Needs vv_finalize_weights (VV_ERR_STATE).  Synchronises. */
+int vv_debug_gemv2(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, int64_t ldx, int map_T, int64_t map_bs, float* y,
+                   int64_t ldy, const float* res, int64_t ldres, int M, int N, int K, int prologue, const float* pro_w, float eps,
+                   int epilogue, const float* epi_a, int64_t epi_lda, int32_t* info, void* stream);
+/* One acoustic-decoder (which = 0: latent [B,64] -> audio [B,3200]) or semantic-encoder (which = 1: audio [B,3200] -> features
+ * [B,semantic_vae_dim]) pass over the current streaming state, launched directly (no graph), with the input of every stage boundary
+ * copied out: after every convolution and every Block1D of the kernel-per-stage path, at the hand-off between the weight-stream program
+ * and that path, and the pass output.  Tap i is [B][T_i][C_i] fp32 (time-major, like the kernels' activations) at float offset
+ * B * sum_{j<i} T_j * C_j of `taps`.  meta (optional) [n_taps][5] = {kind: 0 conv, 1 block, 2 stream hand-off, 3 pass output; stage;
+ * index in stage; T; C}: conv (i, 0) = output of stage i's convolution, block (i, j) = output of block j of stage i, hand-off (s, 0) =
+ * input of stage s, output (n_stages, 0).  Which stages run in the stream program depends on max_batch; meta describes the split that
+ * runs.  Commits the history of `active` rows exactly like vv_codec_decode_frame / vv_semantic_encode_frame (same state, so both may be
+ * interleaved on one context).  taps == NULL: fills meta and returns n_taps, nothing launched.  Too little tap space or a bad `which`:
+ * VV_ERR_INVALID with nothing launched; before vv_finalize_weights: VV_ERR_STATE.  Returns n_taps.  Synchronises. */
+int vv_debug_codec_taps(vv_ctx* ctx, int which, const float* in, const int32_t* active, float* out, float* taps, int64_t taps_floats,
+                        int32_t* meta, void* stream);
 
 int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_out);
 /* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).

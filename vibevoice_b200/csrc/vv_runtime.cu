@@ -214,8 +214,14 @@ static int gemv_occupancy(vv_ctx* c, int smem) {
   return occ;
 }
 
-// y = epi(W * pro(x) + bias); dispatches GEMV (M <= 16) or the tiled GEMM.
-static int linear(const L& l, GemvP p) {
+// which kernel linear() ran (vv_debug_gemv2)
+enum {
+  LIN_GEMV = 0, LIN_RING_RMS_GELU, LIN_RING_RMS_NONE, LIN_RING_GAMMA_RESID, LIN_RING_NONE, LIN_RING_GELU, LIN_RING_RESID, LIN_RING_GENERIC,
+  LIN_MMA, LIN_WGMMA
+};
+
+// y = epi(W * pro(x) + bias); dispatches GEMV (M <= 16) or the tiled GEMM.  info (optional): {LIN_* kernel, split-K factor}.
+static int linear(const L& l, GemvP p, int32_t* info = nullptr) {
   if (p.K % 8 != 0) return fail(VV_ERR_INVALID, "linear: K=%d not a multiple of 8", p.K);
   if (((uintptr_t)p.x & 15) || (p.xmap.rs & 3) || (p.xmap.bs & 3)) return fail(VV_ERR_INVALID, "linear: activation rows must be 16-byte aligned");
   // wgmma path: wide GEMMs that fill the chip with 128-row weight tiles (the all-steps AdaLN modulation GEMM:
@@ -229,6 +235,7 @@ static int linear(const L& l, GemvP p) {
     CK(launch_k(l, split_bf16_kernel, dim3((unsigned)std::min<long long>((n4 + 255) / 256, 1184)), dim3(256), 0, p.x, p.xmap, hi, lo, p.M, p.K));
     CK(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
     CK(launch_k(l, gemm_wgmma_kernel, dim3((p.N + WG_BM - 1) / WG_BM, (p.M + WG_BN - 1) / WG_BN), dim3(128), (size_t)WG_SMEM, p, (const bf16*)hi, (const bf16*)lo));
+    if (info) { info[0] = LIN_WGMMA; info[1] = 1; }
     return 0;
   }
   if (p.M >= MMA_MIN_ROWS) {
@@ -244,17 +251,20 @@ static int linear(const L& l, GemvP p) {
       // the combinations the codec passes use get their own instantiation (FFN1: folded RMSNorm + GELU; FFN2 / transposed convs: plain or
       // gamma-residual, split-K or not); anything else runs the run-time-switched one
       void (*fn)(GemvP) = gemm_mma_ring_kernel<-1, -1>;
-      if (ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<1, EPI_GELU>;
-      else if (ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<1, EPI_NONE>;
-      else if (!ring_rms && p.epi == EPI_GAMMA_RESID) fn = gemm_mma_ring_kernel<0, EPI_GAMMA_RESID>;
-      else if (!ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<0, EPI_NONE>;
-      else if (!ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<0, EPI_GELU>;
-      else if (!ring_rms && p.epi == EPI_RESID) fn = gemm_mma_ring_kernel<0, EPI_RESID>;
+      int which = LIN_RING_GENERIC;
+      if (ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<1, EPI_GELU>, which = LIN_RING_RMS_GELU;
+      else if (ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<1, EPI_NONE>, which = LIN_RING_RMS_NONE;
+      else if (!ring_rms && p.epi == EPI_GAMMA_RESID) fn = gemm_mma_ring_kernel<0, EPI_GAMMA_RESID>, which = LIN_RING_GAMMA_RESID;
+      else if (!ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<0, EPI_NONE>, which = LIN_RING_NONE;
+      else if (!ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<0, EPI_GELU>, which = LIN_RING_GELU;
+      else if (!ring_rms && p.epi == EPI_RESID) fn = gemm_mma_ring_kernel<0, EPI_RESID>, which = LIN_RING_RESID;
       CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MR_SMEM_NORM));
       CK(launch_k(l, fn, dim3(grid), dim3(128), (size_t)(ring_rms ? MR_SMEM_NORM : MR_SMEM), p));
+      if (info) { info[0] = which; info[1] = (int32_t)grid.z; }
       return 0;
     }
     CK(launch_k(l, gemm_mma_kernel, dim3(grid), dim3(128), 0, p));
+    if (info) { info[0] = LIN_MMA; info[1] = (int32_t)grid.z; }
     return 0;
   }
   int MB = p.M <= 1 ? 1 : (p.M <= 2 ? 2 : (p.M <= 4 ? 4 : 8));
@@ -272,6 +282,7 @@ static int linear(const L& l, GemvP p) {
                                                                                                           : gemv_occupancy<8>(l.c, smem);
   int grid = std::min(ntasks, l.c->sm_count * occ);
   if (l.c->gemv_grid_cap) grid = std::min(grid, l.c->gemv_grid_cap);
+  if (info) { info[0] = LIN_GEMV; info[1] = 1; }
   switch (MB) {
     case 1: return launch_gemv_t<1>(l, p, grid, smem);
     case 2: return launch_gemv_t<2>(l, p, grid, smem);
@@ -1795,12 +1806,16 @@ static int stage_ops(StreamBuilder& b, vv_ctx* c, CodecBufs& cb, const std::vect
 
 // decoder front: stem conv + the leading stages with <= 8 rows; *n_front = stages covered (at least stage 0: T = 1, B <= 8 rows), *out_x =
 // where the last one leaves its rows
+static int dec_front_stages(const vv_ctx* c) {
+  int nf = 1;
+  while (nf < c->d.n_stages - 1 && codec_stream_stage(c, c->dec, nf)) ++nf;
+  return nf;
+}
 static int dec_front_prog(vv_ctx* c, const float* latent, const vv_ctx::StreamProg** out, int* n_front, float** out_x) {
   Codec& k = c->dec;
   const auto& d = c->d;
   const int B = d.max_batch;
-  int nf = 1;
-  while (nf < d.n_stages - 1 && codec_stream_stage(c, k, nf)) ++nf;
+  const int nf = dec_front_stages(c);
   *n_front = nf;
   char key[96];
   snprintf(key, sizeof key, "decf:%p", (const void*)latent);
@@ -1877,12 +1892,61 @@ static int enc_back_prog(vv_ctx* c, const float* xin, float* feat, const vv_ctx:
   return 0;
 }
 
-static int enqueue_decode(const L& l, const int32_t* active, float* audio, const vv_ctx::StreamProg& front, int n_front, float* front_x) {
+// ---- stage taps of one codec pass (vv_debug_codec_taps): every stage boundary of the kernel-per-stage path, the hand-off to / from the
+// weight-stream program and the pass output, copied out [B][T][C] in pass order.  Production passes run with no sink.
+enum { TAP_CONV = 0, TAP_BLOCK = 1, TAP_HANDOFF = 2, TAP_OUT = 3 };
+struct TapMeta { int kind, stage, index, T, C; };
+// kind, stage, index: TAP_CONV (i, 0) = output of stage i's convolution; TAP_BLOCK (i, j) = output of block j of stage i; TAP_HANDOFF
+// (s, 0) = input of stage s where the stream program and the kernel-per-stage path meet; TAP_OUT (n_stages, 0) = the pass output
+static void codec_tap_plan(const vv_ctx* c, int which, std::vector<TapMeta>* plan) {
+  const int ns = c->d.n_stages;
+  plan->clear();
+  if (which == 0) {
+    const Codec& k = c->dec;
+    const int nf = dec_front_stages(c);
+    plan->push_back({TAP_HANDOFF, nf, 0, k.T[nf - 1], k.C[nf - 1]});
+    for (int i = nf; i < ns; ++i) {
+      plan->push_back({TAP_CONV, i, 0, k.T[i], k.C[i]});
+      for (int j = 0; j < (int)k.stages[i].size(); ++j) plan->push_back({TAP_BLOCK, i, j, k.T[i], k.C[i]});
+    }
+    plan->push_back({TAP_OUT, ns, 0, k.T[ns - 1], k.convs[ns].Cout});
+  } else {
+    const Codec& k = c->enc;
+    const int stop = enc_back_first(c);
+    for (int i = 0; i < stop; ++i) {
+      plan->push_back({TAP_CONV, i, 0, k.T[i], k.C[i]});
+      for (int j = 0; j < (int)k.stages[i].size(); ++j) plan->push_back({TAP_BLOCK, i, j, k.T[i], k.C[i]});
+    }
+    plan->push_back({TAP_HANDOFF, stop, 0, k.T[stop - 1], k.C[stop - 1]});
+    plan->push_back({TAP_OUT, ns, 0, 1, k.convs[ns].Cout});
+  }
+}
+struct TapSink {
+  std::vector<TapMeta> plan;
+  float* dst = nullptr;        // device, room for B * sum(T * C) floats
+  const float* out = nullptr;  // the pass output buffer (the encoder's is written by its stream program)
+  int B = 0;
+  size_t next = 0;
+  long long off = 0;
+  int put(const L& l, int kind, int stage, int index, const float* src) {
+    if (next >= plan.size() || plan[next].kind != kind || plan[next].stage != stage || plan[next].index != index)
+      return fail(VV_ERR_STATE, "codec taps: tap %zu (kind %d, stage %d, index %d) is not the planned one", next, kind, stage, index);
+    const long long n = (long long)B * plan[next].T * plan[next].C;
+    CK(cudaMemcpyAsync(dst + off, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, l.s));
+    off += n;
+    ++next;
+    return 0;
+  }
+};
+
+static int enqueue_decode(const L& l, const int32_t* active, float* audio, const vv_ctx::StreamProg& front, int n_front, float* front_x,
+                          TapSink* taps = nullptr) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
   Codec& k = c->dec;
   const int B = d.max_batch, ns = d.n_stages;
   RET(launch_stream(l, front));                 // stem + stages [0, n_front) through the weight-stream kernel
+  if (taps) RET(taps->put(l, TAP_HANDOFF, n_front, 0, front_x));
   float *xa = front_x, *xb = c->s_xb;
   for (int i = n_front; i < ns; ++i) {          // i >= 1: every remaining stage starts with its transposed conv
     const ConvL& cv = k.convs[i];
@@ -1893,13 +1957,19 @@ static int enqueue_decode(const L& l, const int32_t* active, float* audio, const
     GemvP p = mk(cv.w, cv.bias, c->s_win, 0, dst, cv.N, B * Tin, cv.N, cv.K);
     p.xmap = xm;
     RET(linear(l, p));
+    if (taps) RET(taps->put(l, TAP_CONV, i, 0, dst));
     xa = dst; xb = (xa == c->s_xa) ? c->s_xb : c->s_xa;
-    for (const Block& b : k.stages[i]) { RET(enqueue_block(l, b, xa, xb, B, k.T[i], d.codec_eps)); std::swap(xa, xb); }
+    for (int j = 0; j < (int)k.stages[i].size(); ++j) {
+      RET(enqueue_block(l, k.stages[i][j], xa, xb, B, k.T[i], d.codec_eps));
+      std::swap(xa, xb);
+      if (taps) RET(taps->put(l, TAP_BLOCK, i, j, xa));
+    }
   }
   const ConvL& hd = k.convs[ns];
   const int T = k.T[ns - 1];
   RET(assemble(l, xa, hd.hist, c->s_win, hd.next, B, T, 6, hd.Cin, nullptr, 0.f, 1.f, 0.f));
   RET(conv_apply(l, hd, c->s_win, audio, B, T, T));
+  if (taps) RET(taps->put(l, TAP_OUT, ns, 0, audio));
   CK(launch_k(l, advance_kernel, dim3(k.n_segs, B, ADV_SLICES), dim3(256), 0, k.segs_dev, active));
   return 0;
 }
@@ -1916,7 +1986,7 @@ static float* encode_front_out(vv_ctx* c, int first) {
   }
   return in_a ? c->s_xa : c->s_xb;
 }
-static int enqueue_encode(const L& l, const float* audio, const int32_t* active, const vv_ctx::StreamProg& back) {
+static int enqueue_encode(const L& l, const float* audio, const int32_t* active, const vv_ctx::StreamProg& back, TapSink* taps = nullptr) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
   Codec& k = c->enc;
@@ -1934,10 +2004,17 @@ static int enqueue_encode(const L& l, const float* audio, const int32_t* active,
       RET(conv_apply(l, cv, c->s_win, xb, B, k.T[i], Tin));
       std::swap(xa, xb);
     }
-    for (const Block& b : k.stages[i]) { RET(enqueue_block(l, b, xa, xb, B, k.T[i], d.codec_eps)); std::swap(xa, xb); }
+    if (taps) RET(taps->put(l, TAP_CONV, i, 0, xa));
+    for (int j = 0; j < (int)k.stages[i].size(); ++j) {
+      RET(enqueue_block(l, k.stages[i][j], xa, xb, B, k.T[i], d.codec_eps));
+      std::swap(xa, xb);
+      if (taps) RET(taps->put(l, TAP_BLOCK, i, j, xa));
+    }
   }
   if (xa != encode_front_out(c, stop)) return fail(VV_ERR_STATE, "encoder hand-off buffer mismatch");
+  if (taps) RET(taps->put(l, TAP_HANDOFF, stop, 0, xa));
   RET(launch_stream(l, back));                  // stages [stop, ns) + head conv through the weight-stream kernel
+  if (taps) RET(taps->put(l, TAP_OUT, d.n_stages, 0, taps->out));
   CK(launch_k(l, advance_kernel, dim3(k.n_segs, B, ADV_SLICES), dim3(256), 0, k.segs_dev, active));
   return 0;
 }
@@ -1977,6 +2054,39 @@ extern "C" int vv_semantic_encode_frame(vv_ctx* c, const float* audio, const int
   const vv_ctx::StreamProg* back;
   RET(enc_back_prog(c, encode_front_out(c, enc_back_first(c)), feat_out, &back));
   return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_encode(l, audio, active, *back); });
+}
+extern "C" int vv_debug_codec_taps(vv_ctx* c, int which, const float* in, const int32_t* active, float* out, float* taps, int64_t taps_floats,
+                                   int32_t* meta, void* stream) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->finalized) return fail(VV_ERR_STATE, "vv_debug_codec_taps: not finalized");
+  if (which != 0 && which != 1) return fail(VV_ERR_INVALID, "vv_debug_codec_taps: which = %d (0 decoder, 1 semantic encoder)", which);
+  TapSink sink;
+  codec_tap_plan(c, which, &sink.plan);
+  const int n = (int)sink.plan.size();
+  long long need = 0;
+  for (int i = 0; i < n; ++i) {
+    const TapMeta& t = sink.plan[i];
+    need += (long long)c->d.max_batch * t.T * t.C;
+    if (meta) { int32_t* m = meta + 5 * i; m[0] = t.kind; m[1] = t.stage; m[2] = t.index; m[3] = t.T; m[4] = t.C; }
+  }
+  if (!taps) return n;
+  if (taps_floats < need) return fail(VV_ERR_INVALID, "vv_debug_codec_taps: %lld floats of tap space, the pass needs %lld", (long long)taps_floats, need);
+  if (!in || !active || !out) return fail(VV_ERR_INVALID, "vv_debug_codec_taps: null input, active set or output");
+  CK(cudaSetDevice(c->device));
+  sink.dst = taps; sink.out = out; sink.B = c->d.max_batch;
+  L l{c, (cudaStream_t)stream};
+  if (which == 0) {
+    const vv_ctx::StreamProg* front; int nf; float* fx;
+    RET(dec_front_prog(c, in, &front, &nf, &fx));
+    RET(enqueue_decode(l, active, out, *front, nf, fx, &sink));
+  } else {
+    const vv_ctx::StreamProg* back;
+    RET(enc_back_prog(c, encode_front_out(c, enc_back_first(c)), out, &back));
+    RET(enqueue_encode(l, in, active, *back, &sink));
+  }
+  CK(cudaStreamSynchronize(l.s));
+  if (sink.next != sink.plan.size()) return fail(VV_ERR_STATE, "vv_debug_codec_taps: the pass made %zu of %d taps", sink.next, n);
+  return n;
 }
 extern "C" int vv_connect(vv_ctx* c, const float* latent, const float* sem, const int32_t* active, float* embeds, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
@@ -2329,6 +2439,32 @@ extern "C" int vv_debug_gemv(vv_ctx* c, const void* w, const float* bias, const 
   p.pro = prologue; p.pro_w = pro_w; p.pro_eps = eps; p.epi = epilogue;
   if (epilogue == EPI_RESID) { p.res = y; p.ldres = N; }
   return linear(l, p);
+}
+
+// linear() with the row map, strides, separate or in-place residual and epilogue operand of the codec's kernel-per-stage GEMMs (see the header)
+extern "C" int vv_debug_gemv2(vv_ctx* c, const void* w, const float* bias, const float* x, int64_t ldx, int map_T, int64_t map_bs, float* y,
+                              int64_t ldy, const float* res, int64_t ldres, int M, int N, int K, int prologue, const float* pro_w, float eps,
+                              int epilogue, const float* epi_a, int64_t epi_lda, int32_t* info, void* stream) {
+  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  if (!w || !x || !y || !info || M < 1 || N < 1 || K < 8) return fail(VV_ERR_INVALID, "vv_debug_gemv2: null operand or empty shape");
+  if (prologue != PRO_NONE && prologue != PRO_RMSNORM && prologue != PRO_SILU) return fail(VV_ERR_INVALID, "vv_debug_gemv2: prologue %d", prologue);
+  if (prologue == PRO_RMSNORM && !pro_w) return fail(VV_ERR_INVALID, "vv_debug_gemv2: RMSNorm needs its weight");
+  const bool has_res = epilogue == EPI_RESID || epilogue == EPI_GATED_RESID || epilogue == EPI_GAMMA_RESID;
+  if (epilogue != EPI_NONE && epilogue != EPI_GELU && epilogue != EPI_SILU && !has_res) return fail(VV_ERR_INVALID, "vv_debug_gemv2: epilogue %d", epilogue);
+  if ((has_res && (!res || ldres < N || ldres > INT32_MAX)) || ((epilogue == EPI_GAMMA_RESID || epilogue == EPI_GATED_RESID) && !epi_a) ||
+      (epilogue == EPI_GATED_RESID && epi_lda < N))
+    return fail(VV_ERR_INVALID, "vv_debug_gemv2: missing residual / epilogue operand");
+  if (ldx < 1 || map_T < 0 || map_bs < 0 || ldy < N || ldy > INT32_MAX) return fail(VV_ERR_INVALID, "vv_debug_gemv2: bad strides");
+  CK(cudaSetDevice(c->device));
+  L l{c, (cudaStream_t)stream};
+  GemvP p = mk((const bf16*)w, bias, x, ldx, y, (int)ldy, M, N, K);
+  if (map_T > 0) { p.xmap.T = map_T; p.xmap.bs = map_bs; }
+  p.pro = prologue; p.pro_w = pro_w; p.pro_eps = eps; p.epi = epilogue;
+  p.epi_a = epi_a; p.epi_lda = epi_lda; p.res = res; p.ldres = (int)ldres;
+  RET(linear(l, p, info));
+  CK(cudaStreamSynchronize(l.s));
+  CKL();
+  return 0;
 }
 
 // builds, runs and frees a one-off stream program (tests); returns the number of stages it ran (after the K split)

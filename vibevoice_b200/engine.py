@@ -389,6 +389,31 @@ class Engine:
     def codec_state_reset(self):
         N.check(self.lib.vv_codec_state_reset(self.h, self.s))
 
+    def codec_taps(self, which: int, rows):
+        """One decoder (which = 0: `latent` -> `audio`) or semantic-encoder (which = 1: `audio` -> `feat`) pass with every stage boundary
+        copied out (`vv_debug_codec_taps`, tests).  `rows` become the active set and commit their history, as in `codec_decode` /
+        `semantic_encode`.  Returns [(meta, tap)]: meta = (kind, stage, index, T, C), tap = [B, T, C] fp32 CPU tensor."""
+        src, dst = (self.latent, self.audio) if which == 0 else (self.audio, self.feat)
+        n = N.check(self.lib.vv_debug_codec_taps(self.h, int(which), None, None, None, None, 0, None, None), "vv_debug_codec_taps")
+        meta = np.zeros((n, 5), dtype=np.int32)
+        N.check(self.lib.vv_debug_codec_taps(self.h, int(which), None, None, None, None, 0, N.iptr(meta), None), "vv_debug_codec_taps")
+        sizes = [self.B * int(t) * int(c) for t, c in meta[:, 3:]]
+        self.active_h.zero_()
+        for r in rows:
+            self.active_h[r] = 1
+        with torch.cuda.stream(self.stream):
+            self.active.copy_(self.active_h, non_blocking=True)
+            taps = torch.empty(sum(sizes), dtype=torch.float32, device=self.device)
+            N.check(self.lib.vv_debug_codec_taps(self.h, int(which), C.c_void_p(src.data_ptr()), C.c_void_p(self.active.data_ptr()),
+                                                 C.c_void_p(dst.data_ptr()), C.c_void_p(taps.data_ptr()), taps.numel(), None, self.s),
+                    "vv_debug_codec_taps")
+        taps = taps.cpu()
+        out, off = [], 0
+        for m, sz in zip(meta.tolist(), sizes):
+            out.append((tuple(m), taps[off:off + sz].view(self.B, m[3], m[4])))
+            off += sz
+        return out
+
     def launch_count(self) -> int:
         return int(self.lib.vv_launch_count(self.h))
 
