@@ -92,7 +92,8 @@ int64_t vv_weight_bytes(vv_ctx* ctx, int which); /* 0 lm, 1 head-per-step, 2 con
 /* ---- paged KV cache (replaces HF DynamicCache, modeling_vibevoice_inference.py:303, 556-562) -- *
  * 2B sequences share one pool of pages (64 tokens each, all layers); pages return to the pool when vv_kv_set_len shrinks a sequence. */
 int vv_kv_init(vv_ctx* ctx, int64_t n_pages);   /* calling it again re-sizes the pool: every sequence is dropped, LM graphs re-captured */
-int vv_kv_reserve(vv_ctx* ctx, int seq, int64_t n_tokens, void* stream); /* make positions < n_tokens addressable */
+int vv_kv_reserve(vv_ctx* ctx, int seq, int64_t n_tokens, void* stream); /* make positions < n_tokens addressable; pages it adds
+                                                                            arrive with K and V zero in every layer */
 int vv_kv_set_len(vv_ctx* ctx, int seq, int64_t len, void* stream);      /* e.g. 0 = negative-stream refresh (:549-565) */
 int vv_kv_write(vv_ctx* ctx, int seq, int layer, int64_t pos0, int64_t n_tokens,
                 const void* k_bf16, const void* v_bf16, void* stream);   /* prefill hand-off: [n_tokens, kv_heads, head_dim] */

@@ -1292,7 +1292,16 @@ extern "C" int64_t vv_kv_len(vv_ctx* c, int seq) { return (c && seq >= 0 && seq 
 // page-table entries travel BY VALUE in the launch arguments: pages return to the free list when a sequence shrinks, so an entry can be
 // rewritten while copies of its previous value are still queued on the stream -- an asynchronous copy out of a host mirror would race
 struct PageVals { int v[32]; };
-__global__ void page_table_set_kernel(int* dst, PageVals pv, int n) { if ((int)threadIdx.x < n) dst[threadIdx.x] = pv.v[threadIdx.x]; }
+// block (i, layer) zeroes the K and V rows of page pv.v[i] in that layer; block (0, 0) also writes the page-table entries.  A page handed out
+// again can hold a previous owner's entries, non-finite ones included, in the slots past the new owner's length: attention masks their
+// scores, but its P V product would still take 0 * NaN = NaN from them.  Zeroing here, once per page grant, keeps that off the decode step.
+__global__ void page_grant_kernel(int* dst, PageVals pv, int n, bf16* kpool, bf16* vpool, size_t per_layer, size_t page_elems) {
+  if (blockIdx.x == 0 && blockIdx.y == 0 && (int)threadIdx.x < n) dst[threadIdx.x] = pv.v[threadIdx.x];
+  const size_t o = per_layer * blockIdx.y + (size_t)pv.v[blockIdx.x] * page_elems;
+  uint4* k = reinterpret_cast<uint4*>(kpool + o);
+  uint4* v = reinterpret_cast<uint4*>(vpool + o);
+  for (size_t i = threadIdx.x; i < page_elems / 8; i += blockDim.x) { k[i] = make_uint4(0u, 0u, 0u, 0u); v[i] = make_uint4(0u, 0u, 0u, 0u); }
+}
 
 extern "C" int vv_kv_reserve(vv_ctx* c, int seq, int64_t n_tokens, void* stream) {
   if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
@@ -1310,7 +1319,10 @@ extern "C" int vv_kv_reserve(vv_ctx* c, int seq, int64_t n_tokens, void* stream)
     PageVals pv;
     const int n = (int)std::min<size_t>(32, pg.size() - first);
     for (int i = 0; i < 32; ++i) pv.v[i] = i < n ? pg[first + i] : 0;
-    page_table_set_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(c->page_table_dev + (size_t)seq * c->max_pages + first, pv, n);
+    const auto& d = c->d;
+    const size_t page_elems = (size_t)d.num_kv_heads * KV_PAGE * d.head_dim;
+    page_grant_kernel<<<dim3(n, d.num_layers), 256, 0, (cudaStream_t)stream>>>(c->page_table_dev + (size_t)seq * c->max_pages + first, pv, n,
+                                                                                 c->kpool, c->vpool, (size_t)c->n_pages * page_elems, page_elems);
     CKL();
     c->launches++;
     first += n;
