@@ -216,6 +216,22 @@ int vv_debug_gemv2(vv_ctx* ctx, const void* w_bf16, const float* bias, const flo
  * VV_ERR_INVALID with nothing launched; before vv_finalize_weights: VV_ERR_STATE.  Returns n_taps.  Synchronises. */
 int vv_debug_codec_taps(vv_ctx* ctx, int which, const float* in, const int32_t* active, float* out, float* taps, int64_t taps_floats,
                         int32_t* meta, void* stream);
+/* vv_diffusion_sample launched directly (no graph) with every solver block's result copied out.  The preamble is the production one
+ * (cond_proj, the conditioning kernel, the all-steps modulation GEMM); the sampler program then runs as one launch per block, each built by
+ * the production builder and checked stage by stage (kernel variant, K split) against the production program: proj(-1), then per step i
+ * head layer li = 0 .. L-1, the final layer and proj(i) (CFG + DPM-Solver++ update of step i, then noisy_images_proj).  SDE step noise
+ * and the device-held CFG scale are used as in production.  Tap j is [rows_j][cols_j] fp32 at float offset sum_{k<j} rows_k * cols_k of
+ * `taps`; meta (optional) [n_taps][7] = {kind, step, layer, rows, cols, kernel, split}, in this order:
+ *   kind 0: silu(t_embedder.mlp.0(t)) [N][H]      1: t embedding temb [N][H]  (both as left by vv_set_diffusion_steps)
+ *   kind 2: cond_proj(cond) [2B][H]               3: AdaLN modulation of every step [N * 2B][(3L+2)H]
+ *   then kind 6 z_0 (= noise), 7 x0 (zeros), 8 x [2B][H] for step -1, and per step i: kind 4 residual stream after head layer `layer`
+ *   [2B][H], 5 head output v [2B][64], 6 z_{i+1} [B][64], 7 x0_i [B][64], 8 x = noisy_images_proj(z_{i+1}) [2B][H]; last, kind 9 latent_out.
+ * kernel / split: kinds 0-3 = the {kernel, split-K factor} linear() ran (numbering as vv_debug_gemv2); block taps = the stream-kernel variant
+ * and the number of stages (after the K split) of the block that wrote them.  taps == NULL: fills meta (kernel -1) and returns n_taps,
+ * nothing launched.  Too little tap space: VV_ERR_INVALID with nothing launched; before vv_set_diffusion_steps (or SDE without step noise):
+ * VV_ERR_STATE.  Returns n_taps.  Synchronises. */
+int vv_debug_sampler_taps(vv_ctx* ctx, const float* cond, const float* noise, float cfg_scale, float* latent_out, float* taps,
+                          int64_t taps_floats, int32_t* meta, void* stream);
 
 int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_out);
 /* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).

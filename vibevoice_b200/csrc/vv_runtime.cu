@@ -114,6 +114,7 @@ struct vv_ctx {
   bf16 *h_noisy = nullptr, *h_cond = nullptr, *h_t0 = nullptr, *h_t2 = nullptr, *h_mod = nullptr, *h_final = nullptr;
   std::vector<HeadLayer> head;
   int n_steps = 0; float* temb = nullptr; float* tfreqs = nullptr;
+  int32_t temb_info[2][2] = {{-1, 0}, {-1, 0}};   // {kernel, split-K} linear() ran for t_embedder.mlp.0 / .2 (vv_debug_sampler_taps)
   std::vector<DpmCoef> coef_host; int coef_version = 0;
   bool sde = false; const float* step_noise = nullptr;   // sde-dpmsolver++: per-step variance noise [n_steps][B][64] (vv_set_step_noise)
   // connectors
@@ -1595,9 +1596,9 @@ static int set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, c
   L l{c, s};
   GemvP p = mk(c->h_t0, nullptr, c->s_tfeat, 256, c->s_t1, H, n_steps, H, 256);
   p.epi = EPI_SILU;
-  RET(linear(l, p));
+  RET(linear(l, p, c->temb_info[0]));
   p = mk(c->h_t2, nullptr, c->s_t1, H, c->temb, H, n_steps, H, H);
-  RET(linear(l, p));
+  RET(linear(l, p, c->temb_info[1]));
   CK(cudaStreamSynchronize(s));
   c->n_steps = n_steps;
   // programs captured with another step count are stale
@@ -1620,16 +1621,17 @@ static int set_cfg(vv_ctx* c, float cfg, cudaStream_t s) {
 // The N-step sampler as ONE weight-stream program (vv_stream.cuh): per step 4 x (gate/up with AdaLN prologue -> raw sums; down with SwiGLU
 // prologue, gated-residual epilogue) + final layer + noisy_images_proj whose prologue is the CFG / DPM-Solver++ update.  10 grid barriers
 // per step instead of 10 kernels, and the TMA ring keeps streaming head weights across all of them.
-static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out, const vv_ctx::StreamProg** out) {
-  char key[256];
-  snprintf(key, sizeof key, "samp:%p:%p:%d:%d:%p:%d", (const void*)noise, (void*)latent_out, c->n_steps, (int)c->sde, (const void*)c->step_noise,
-           c->coef_version);       // solver coefficients are baked into the program
-  auto it = c->sprogs.find(key);
-  if (it != c->sprogs.end()) { *out = &it->second; return 0; }
+// The program is a sequence of blocks: block 0 = proj(-1) (x = noisy_images_proj(initial noise)); then per step i, from block
+// 1 + i (L + 2): head layer li = 0 .. L-1 (gate/up + down), the final layer, proj(i).  sampler_build emits blocks [blk0, blk1) only.  Every
+// value one block hands to the next lives in global memory (s_hx, the gu double buffer, s_v, the s_z / s_x0 parity buffers, s_mod) and the
+// zero-fill jobs ride on earlier stages, so the blocks launched one after another compute what the whole program does (vv_debug_sampler_taps).
+static int sampler_blocks(const vv_ctx* c) { return 1 + c->n_steps * (c->d.head_layers + 2); }
+static int sampler_build(StreamBuilder& b, const float* noise, float* latent_out, int blk0, int blk1) {
+  vv_ctx* c = b.c;
   const auto& d = c->d;
   const int H = d.hidden_size, F = d.head_ffn_dim, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = c->n_steps;
   const long long modld = (long long)(3 * LH + 2) * H;
-  StreamBuilder b(c);
+  auto in = [&](int blk) { return blk >= blk0 && blk < blk1; };
   auto dpm = [&](int i) {
     SDpm o;
     memset(&o, 0, sizeof o);
@@ -1650,11 +1652,15 @@ static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out,
     return 0;
   };
   float* gu[2] = {c->s_hgu, c->s_hgu + (size_t)M * 2 * F};
-  RET(proj(-1, false));
-  b.ops.back().init_dst = gu[0]; b.ops.back().init_n = (long long)M * 2 * F;
+  if (in(0)) {
+    RET(proj(-1, false));
+    b.ops.back().init_dst = gu[0]; b.ops.back().init_n = (long long)M * 2 * F;
+  }
   for (int i = 0; i < N; ++i) {
     const float* mod = c->s_mod + (size_t)i * M * modld;
+    const int base = 1 + i * (LH + 2);
     for (int li = 0; li < LH; ++li) {
+      if (!in(base + li)) continue;
       const HeadLayer& hl = c->head[li];
       SOp* o;
       RET(b.gemv(hl.wgu, nullptr, c->s_hx, H, gu[li & 1], 2 * F, M, 2 * F, H, true, &o));
@@ -1665,12 +1671,25 @@ static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out,
       o->pro = SP_SWIGLU; o->alpha_kind = SA_GATE; o->alpha = mod + (size_t)li * 3 * H + 2 * H; o->lda = modld;
       if (li == 0) { o->init_dst = c->s_v; o->init_n = (long long)M * 64; }        // final layer of this step accumulates into s_v
     }
-    SOp* o;
-    RET(b.gemv(c->h_final, nullptr, c->s_hx, H, c->s_v, 64, M, 64, H, true, &o));
-    o->pro = SP_ADALN; o->pro_w = nullptr; o->pro_eps = d.head_rms_eps;
-    o->pro_shift = mod + (size_t)LH * 3 * H; o->pro_scale = mod + (size_t)LH * 3 * H + H; o->pro_ld = modld;
-    RET(proj(i, true));
+    if (in(base + LH)) {
+      SOp* o;
+      RET(b.gemv(c->h_final, nullptr, c->s_hx, H, c->s_v, 64, M, 64, H, true, &o));
+      o->pro = SP_ADALN; o->pro_w = nullptr; o->pro_eps = d.head_rms_eps;
+      o->pro_shift = mod + (size_t)LH * 3 * H; o->pro_scale = mod + (size_t)LH * 3 * H + H; o->pro_ld = modld;
+    }
+    if (in(base + LH + 1)) RET(proj(i, true));
   }
+  if (!b.ops.empty()) b.ops.front().sync_before = 0;     // the first stage of a launch waits for nothing
+  return 0;
+}
+static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out, const vv_ctx::StreamProg** out) {
+  char key[256];
+  snprintf(key, sizeof key, "samp:%p:%p:%d:%d:%p:%d", (const void*)noise, (void*)latent_out, c->n_steps, (int)c->sde, (const void*)c->step_noise,
+           c->coef_version);       // solver coefficients are baked into the program
+  auto it = c->sprogs.find(key);
+  if (it != c->sprogs.end()) { *out = &it->second; return 0; }
+  StreamBuilder b(c);
+  RET(sampler_build(b, noise, latent_out, 0, sampler_blocks(c)));
   vv_ctx::StreamProg pr;
   RET(finish_stream(b, &pr));
   it = c->sprogs.emplace(key, pr).first;
@@ -1678,7 +1697,9 @@ static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out,
   return 0;
 }
 
-static int enqueue_diffusion(const L& l, const float* cond, const vv_ctx::StreamProg& sprog) {
+// Everything the samp: program reads besides its inputs: cond_proj, the conditioning kernel and the all-steps AdaLN modulation GEMM.
+// info_cond / info_mod (optional): {kernel, split-K} linear() ran for cond_proj / the modulation GEMM.
+static int diffusion_preamble(const L& l, const float* cond, int32_t* info_cond = nullptr, int32_t* info_mod = nullptr) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
   const int H = d.hidden_size, M = 2 * d.max_batch, LH = d.head_layers, N = c->n_steps;
@@ -1686,7 +1707,7 @@ static int enqueue_diffusion(const L& l, const float* cond, const vv_ctx::Stream
   const int modld = (3 * LH + 2) * H;
   if (c->sde && !c->step_noise) return fail(VV_ERR_STATE, "sde-dpmsolver++ needs vv_set_step_noise before sampling");
   GemvP p = mk(c->h_cond, nullptr, cond, H, c->s_condp, H, M, H, H);
-  RET(linear(l, p));
+  RET(linear(l, p, info_cond));
   {
     const long long n = (long long)N * M * H;
     CK(launch_k(l, head_cond_prep_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, c->s_condp, c->temb, c->s_call, N, M, H));
@@ -1694,7 +1715,12 @@ static int enqueue_diffusion(const L& l, const float* cond, const vv_ctx::Stream
   // AdaLN modulation of ALL steps and layers in one tensor-core GEMM: c_all [N*M, H] x W_mod^T -> [N*M, (3L+2)H].
   // (the reference recomputes Linear(silu(c)) inside every head call, diffusion_head.py:159, 185; c depends only on (cond, t_i))
   p = mk(c->h_mod, nullptr, c->s_call, H, c->s_mod, modld, N * M, modld, H);
-  RET(linear(l, p));
+  RET(linear(l, p, info_mod));
+  return 0;
+}
+
+static int enqueue_diffusion(const L& l, const float* cond, const vv_ctx::StreamProg& sprog) {
+  RET(diffusion_preamble(l, cond));
   return launch_stream(l, sprog);
 }
 
@@ -1709,6 +1735,121 @@ extern "C" int vv_diffusion_sample(vv_ctx* c, const float* cond, const float* no
   const vv_ctx::StreamProg* sprog;      // built outside stream capture (it allocates and copies)
   RET(sampler_stream_prog(c, noise, latent_out, &sprog));
   return run_cached(c, key, (cudaStream_t)stream, [&](const L& l) { return enqueue_diffusion(l, cond, *sprog); });
+}
+
+// ---- solver-step taps of the sampler (vv_debug_sampler_taps): the preamble's outputs, then what every block of the samp: program leaves
+// behind, copied out in order.  block = the sampler block after which the tap is copied (-1: before the first).
+enum { STAP_THID = 0, STAP_TEMB, STAP_COND, STAP_MOD, STAP_LAYER, STAP_V, STAP_Z, STAP_X0, STAP_HX, STAP_LATENT };
+struct SampTap { int kind, step, layer, rows, cols; const float* src; int block; };
+static void sampler_tap_plan(const vv_ctx* c, float* latent_out, std::vector<SampTap>* plan) {
+  const auto& d = c->d;
+  const int H = d.hidden_size, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = c->n_steps, modld = (3 * LH + 2) * H;
+  plan->clear();
+  plan->push_back({STAP_THID, -1, -1, N, H, c->s_t1, -1});
+  plan->push_back({STAP_TEMB, -1, -1, N, H, c->temb, -1});
+  plan->push_back({STAP_COND, -1, -1, M, H, c->s_condp, -1});
+  plan->push_back({STAP_MOD, -1, -1, N * M, modld, c->s_mod, -1});
+  auto proj = [&](int i, int blk) {             // proj(i) writes z_{i+1} and x0_i into parity slot (i + 1) & 1 (i = -1: slot 0)
+    const size_t slot = (size_t)((i + 1) & 1) * B * 64;
+    plan->push_back({STAP_Z, i, -1, B, 64, c->s_z + slot, blk});
+    plan->push_back({STAP_X0, i, -1, B, 64, c->s_x0 + slot, blk});
+    plan->push_back({STAP_HX, i, -1, M, H, c->s_hx, blk});
+  };
+  proj(-1, 0);
+  for (int i = 0; i < N; ++i) {
+    const int base = 1 + i * (LH + 2);
+    for (int li = 0; li < LH; ++li) plan->push_back({STAP_LAYER, i, li, M, H, c->s_hx, base + li});
+    plan->push_back({STAP_V, i, -1, M, 64, c->s_v, base + LH});
+    proj(i, base + LH + 1);
+  }
+  plan->push_back({STAP_LATENT, N - 1, -1, B, 64, latent_out, sampler_blocks(c) - 1});
+}
+// the fields that make two stages compute the same thing (the tensor-map and op-array addresses differ between programs)
+static bool same_stage(const SOp& a, const SOp& b) {
+  return a.kind == b.kind && a.M == b.M && a.N == b.N && a.K == b.K && a.nB == b.nB && a.k0 == b.k0 && a.krow == b.krow && a.pro == b.pro &&
+         a.x == b.x && a.ldx == b.ldx && a.pro_w == b.pro_w && a.pro_shift == b.pro_shift && a.pro_scale == b.pro_scale && a.y == b.y &&
+         a.ldy == b.ldy && a.alpha_kind == b.alpha_kind && a.alpha == b.alpha && a.store == b.store && a.init_dst == b.init_dst &&
+         a.init_n == b.init_n && a.dpm.z_in == b.dpm.z_in && a.dpm.z_out == b.dpm.z_out && a.dpm.x0_in == b.dpm.x0_in &&
+         a.dpm.x0_out == b.dpm.x0_out && a.dpm.v == b.dpm.v && a.dpm.noise == b.dpm.noise && a.dpm.step_noise == b.dpm.step_noise &&
+         a.dpm.latent_out == b.dpm.latent_out && a.dpm.step == b.dpm.step && memcmp(&a.dpm.c, &b.dpm.c, sizeof a.dpm.c) == 0;
+}
+extern "C" int vv_debug_sampler_taps(vv_ctx* c, const float* cond, const float* noise, float cfg, float* latent_out, float* taps,
+                                     int64_t taps_floats, int32_t* meta, void* stream) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->finalized) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: not finalized");
+  if (c->n_steps < 1) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: vv_set_diffusion_steps not called");
+  std::vector<SampTap> plan;
+  sampler_tap_plan(c, latent_out, &plan);
+  const int n = (int)plan.size();
+  long long need = 0;
+  for (int i = 0; i < n; ++i) {
+    const SampTap& t = plan[i];
+    need += (long long)t.rows * t.cols;
+    if (meta) { int32_t* m = meta + 7 * i; m[0] = t.kind; m[1] = t.step; m[2] = t.layer; m[3] = t.rows; m[4] = t.cols; m[5] = -1; m[6] = 0; }
+  }
+  if (!taps) return n;
+  if (taps_floats < need) return fail(VV_ERR_INVALID, "vv_debug_sampler_taps: %lld floats of tap space, the sampler needs %lld", (long long)taps_floats, need);
+  if (!cond || !noise || !latent_out) return fail(VV_ERR_INVALID, "vv_debug_sampler_taps: null condition, noise or latent");
+  if (c->sde && !c->step_noise) return fail(VV_ERR_STATE, "sde-dpmsolver++ needs vv_set_step_noise before sampling");
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  // production's own program (cached under its production key, as vv_diffusion_sample would): every block must run on its kernel variant
+  // and be exactly its stages, K split included
+  const vv_ctx::StreamProg* full;
+  RET(sampler_stream_prog(c, noise, latent_out, &full));
+  std::vector<SOp> full_ops(full->n_ops);
+  CK(cudaMemcpy(full_ops.data(), full->ops, full_ops.size() * sizeof(SOp), cudaMemcpyDeviceToHost));
+  const int nb = sampler_blocks(c);
+  std::vector<vv_ctx::StreamProg> progs(nb);
+  auto release = [&]() { for (auto& p : progs) { if (p.ops) dfree(c, &p.ops); if (p.tmaps) dfree(c, &p.tmaps); } };
+  int rc = 0, at = 0;
+  for (int k = 0; k < nb && rc == 0; ++k) {
+    StreamBuilder b(c);
+    rc = sampler_build(b, noise, latent_out, k, k + 1);
+    if (rc == 0) rc = finish_stream(b, &progs[k]);
+    if (rc == 0 && progs[k].variant != full->variant)
+      rc = fail(VV_ERR_STATE, "vv_debug_sampler_taps: block %d runs on kernel variant %d, the program on %d", k, progs[k].variant, full->variant);
+    for (int j = 0; rc == 0 && j < (int)b.ops.size(); ++j, ++at)
+      if (at >= full->n_ops || !same_stage(b.ops[j], full_ops[at]) || (j > 0 && b.ops[j].sync_before != full_ops[at].sync_before))
+        rc = fail(VV_ERR_STATE, "vv_debug_sampler_taps: stage %d of block %d is not stage %d of the program", j, k, at);
+  }
+  if (rc == 0 && at != full->n_ops) rc = fail(VV_ERR_STATE, "vv_debug_sampler_taps: the blocks have %d stages, the program %d", at, full->n_ops);
+  if (rc < 0) { release(); return rc; }
+  int32_t info[2][2] = {{-1, 0}, {-1, 0}};      // cond_proj, modulation GEMM
+  L l{c, s};
+  size_t t = 0;
+  long long off = 0;
+  auto put = [&](int blk) -> int {
+    for (; t < plan.size() && plan[t].block == blk; ++t) {
+      const long long cnt = (long long)plan[t].rows * plan[t].cols;
+      CK(cudaMemcpyAsync(taps + off, plan[t].src, (size_t)cnt * sizeof(float), cudaMemcpyDeviceToDevice, s));
+      off += cnt;
+    }
+    return 0;
+  };
+  rc = set_cfg(c, cfg, s);
+  if (rc == 0) rc = diffusion_preamble(l, cond, info[0], info[1]);
+  if (rc == 0) rc = put(-1);
+  for (int k = 0; k < nb && rc == 0; ++k) {
+    rc = launch_stream(l, progs[k]);
+    if (rc == 0) rc = put(k);
+  }
+  if (rc == 0 && cudaStreamSynchronize(s) != cudaSuccess) rc = fail(VV_ERR_CUDA, "vv_debug_sampler_taps: %s", cudaGetErrorString(cudaGetLastError()));
+  release();
+  if (rc < 0) return rc;
+  if (c->st_diag_host[0]) return fail(VV_ERR_CUDA, "stream kernel watchdog: code %u cta %u thread %u a %u b %u c %u", c->st_diag_host[0], c->st_diag_host[1],
+                                      c->st_diag_host[2], c->st_diag_host[3], c->st_diag_host[4], c->st_diag_host[5]);
+  if (t != plan.size()) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: copied %zu of %d taps", t, n);
+  if (meta)
+    for (int i = 0; i < n; ++i) {
+      int32_t* m = meta + 7 * i;
+      const SampTap& p = plan[i];
+      const int32_t* ki = p.kind == STAP_THID ? c->temb_info[0] : p.kind == STAP_TEMB ? c->temb_info[1] : p.kind == STAP_COND ? info[0]
+                        : p.kind == STAP_MOD ? info[1] : nullptr;
+      if (ki) { m[5] = ki[0]; m[6] = ki[1]; }
+      else { m[5] = progs[p.block].variant; m[6] = progs[p.block].n_ops; }    // progs' fields outlive release(): only the device arrays go
+    }
+  return n;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -414,6 +414,26 @@ class Engine:
             off += sz
         return out
 
+    def sampler_taps(self, cfg_scale: float):
+        """`diffusion_sample` (`hidden` -> `latent`, with `noise`) with every solver block's result copied out (`vv_debug_sampler_taps`,
+        tests).  Returns [(meta, tap)]: meta = (kind, step, layer, rows, cols, kernel, split), tap = [rows, cols] fp32 CPU tensor."""
+        P = lambda t: C.c_void_p(t.data_ptr())
+        call = lambda taps, n, meta, s: self.lib.vv_debug_sampler_taps(self.h, P(self.hidden), P(self.noise), float(cfg_scale), P(self.latent),
+                                                                        taps, n, meta, s)
+        n = N.check(call(None, 0, None, None), "vv_debug_sampler_taps")
+        meta = np.zeros((n, 7), dtype=np.int32)
+        N.check(call(None, 0, N.iptr(meta), None), "vv_debug_sampler_taps")
+        sizes = [int(r) * int(c) for r, c in meta[:, 3:5]]
+        with torch.cuda.stream(self.stream):
+            taps = torch.empty(sum(sizes), dtype=torch.float32, device=self.device)
+            N.check(call(P(taps), taps.numel(), N.iptr(meta), self.s), "vv_debug_sampler_taps")
+        taps = taps.cpu()
+        out, off = [], 0
+        for m, sz in zip(meta.tolist(), sizes):
+            out.append((tuple(m), taps[off:off + sz].view(m[3], m[4])))
+            off += sz
+        return out
+
     def launch_count(self) -> int:
         return int(self.lib.vv_launch_count(self.h))
 
