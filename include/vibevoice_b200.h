@@ -232,6 +232,17 @@ int vv_debug_codec_taps(vv_ctx* ctx, int which, const float* in, const int32_t* 
  * VV_ERR_STATE.  Returns n_taps.  Synchronises. */
 int vv_debug_sampler_taps(vv_ctx* ctx, const float* cond, const float* noise, float cfg_scale, float* latent_out, float* taps,
                           int64_t taps_floats, int32_t* meta, void* stream);
+/* Decoder layer `layer` of vv_lm_prefill alone, over n rows of sequence `seq` at positions [pos0, pos0 + n), from the fp32 residual input
+ * x_in [n][H] (device), with what each of its kernels left copied out.  It runs the kernels vv_lm_prefill runs for that layer, in the same
+ * chunks of the same workspace rule, reserves the same pages and writes the layer's K/V into the pool.  hidden_last (optional, [H] fp32):
+ * the final-norm hidden state of the last output row, as vv_lm_prefill computes it.  Tap k is [n][cols_k] at byte offset
+ * sum_{j<k} n * cols_j * bytes_j of `taps`; meta (optional) [7][3] = {kind, bytes per element, cols}, kinds in this order:
+ *   0 norm1 bf16 [n][H]   1 Q after bias and RoPE bf16 [n][nq]   2 attention output bf16 [n][nq]   3 residual after the o-projection
+ *   fp32 [n][H]   4 norm2 bf16 [n][H]   5 silu(gate) * up bf16 [n][I]   6 layer output fp32 [n][H].
+ * taps == NULL: fills meta and returns 7, nothing launched.  Errors: those of vv_lm_prefill, a bad layer -> VV_ERR_INVALID, too little tap
+ * space -> VV_ERR_INVALID, all with nothing launched.  Returns 7.  Synchronises. */
+int vv_debug_prefill_taps(vv_ctx* ctx, int seq, int64_t pos0, int64_t n, int layer, const float* x_in, float* hidden_last, void* workspace,
+                          int64_t workspace_bytes, void* taps, int64_t taps_bytes, int32_t* meta, void* stream);
 
 int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_out);
 /* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).

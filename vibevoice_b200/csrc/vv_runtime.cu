@@ -2447,83 +2447,164 @@ extern "C" int64_t vv_lm_prefill_workspace(vv_ctx* c, int64_t n_tokens) {
   return pf_bytes(c, 64);
 }
 
-extern "C" int vv_lm_prefill(vv_ctx* c, int seq, int64_t pos0, int64_t n, const float* embeds, float* hidden_last, void* workspace,
-                             int64_t workspace_bytes, void* stream) {
-  RET(pf_check(c, n));
-  if (!embeds || !hidden_last || !workspace) return fail(VV_ERR_INVALID, "vv_lm_prefill: null argument");
-  if ((uintptr_t)workspace & 255) return fail(VV_ERR_INVALID, "vv_lm_prefill: workspace must be 256-byte aligned");
-  if (((uintptr_t)embeds & 15) || ((uintptr_t)hidden_last & 15)) return fail(VV_ERR_INVALID, "vv_lm_prefill: embeds / hidden_last must be 16-byte aligned");
+// the checks and page reservation vv_lm_prefill and vv_debug_prefill_taps share; *R = rows per chunk
+static int pf_begin(vv_ctx* c, const char* who, int seq, int64_t pos0, int64_t n, void* workspace, int64_t workspace_bytes, void* stream,
+                    long long* R) {
+  if ((uintptr_t)workspace & 255) return fail(VV_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
   const long long need = pf_bytes(c, 64);
   if (workspace_bytes < need)
-    return fail(VV_ERR_INVALID, "vv_lm_prefill: workspace of %lld bytes is below the minimum %lld", (long long)workspace_bytes, need);
-  if (!c->kpool) return fail(VV_ERR_STATE, "vv_lm_prefill: KV pool not initialised (vv_kv_init)");
+    return fail(VV_ERR_INVALID, "%s: workspace of %lld bytes is below the minimum %lld", who, (long long)workspace_bytes, need);
+  if (!c->kpool) return fail(VV_ERR_STATE, "%s: KV pool not initialised (vv_kv_init)", who);
   const auto& d = c->d;
-  if (seq < 0 || seq >= 2 * d.max_batch) return fail(VV_ERR_INVALID, "vv_lm_prefill: bad seq %d", seq);
+  if (seq < 0 || seq >= 2 * d.max_batch) return fail(VV_ERR_INVALID, "%s: bad seq %d", who, seq);
   if (pos0 < 0 || pos0 + n > d.max_position_embeddings)
-    return fail(VV_ERR_INVALID, "vv_lm_prefill: positions [%lld, %lld) outside [0, %d)", (long long)pos0, (long long)(pos0 + n), d.max_position_embeddings);
+    return fail(VV_ERR_INVALID, "%s: positions [%lld, %lld) outside [0, %d)", who, (long long)pos0, (long long)(pos0 + n), d.max_position_embeddings);
   {
     const int64_t needp = (pos0 + n + KV_PAGE - 1) / KV_PAGE, have = (int64_t)c->seq_pages[seq].size();
     if (needp > c->max_pages || needp - have > (int64_t)c->free_pages.size())
-      return fail(VV_ERR_NOMEM, "vv_lm_prefill: KV page pool too small (seq %d needs %lld pages, holds %lld, %lld free)", seq, (long long)needp,
+      return fail(VV_ERR_NOMEM, "%s: KV page pool too small (seq %d needs %lld pages, holds %lld, %lld free)", who, seq, (long long)needp,
                   (long long)have, (long long)c->free_pages.size());
   }
   CK(cudaSetDevice(c->device));
   RET(vv_kv_reserve(c, seq, pos0 + n, stream));
   // rows per chunk: the largest multiple of 64 the workspace holds, at most the prompt (rounded up) and 65535 GEMM row tiles
-  long long R = std::min<long long>((n + 63) & ~63ll, 65535ll * PF_BM);
-  while (R > 64 && pf_bytes(c, R) > workspace_bytes) R -= 64;
+  *R = std::min<long long>((n + 63) & ~63ll, 65535ll * PF_BM);
+  while (*R > 64 && pf_bytes(c, *R) > workspace_bytes) *R -= 64;
+  return 0;
+}
+
+// ---- per-kernel taps of one prefill layer (vv_debug_prefill_taps): what each kernel of the layer left, [n][cols] per tap, back to back.
+// Production chunks run with no sink.
+enum { PT_NORM1 = 0, PT_Q, PT_ATTN, PT_RESID1, PT_NORM2, PT_SWIGLU, PT_OUT, PT_COUNT };
+struct PrefillTaps {
+  unsigned char* dst = nullptr;  // device
+  long long off[PT_COUNT];       // byte offset of tap k
+  int cols[PT_COUNT], esz[PT_COUNT];
+  long long c0 = 0;              // first row of the chunk being run
+  PrefillTaps(const vv_ctx* c, long long n) {
+    const auto& d = c->d;
+    const int nq = d.num_q_heads * d.head_dim;
+    const int cc[PT_COUNT] = {d.hidden_size, nq, nq, d.hidden_size, d.hidden_size, d.intermediate_size, d.hidden_size};
+    const int ee[PT_COUNT] = {2, 2, 2, 4, 2, 2, 4};
+    long long o = 0;
+    for (int k = 0; k < PT_COUNT; ++k) { cols[k] = cc[k]; esz[k] = ee[k]; off[k] = o; o += n * cc[k] * ee[k]; }
+  }
+  long long bytes(long long n) const { return off[PT_COUNT - 1] + n * cols[PT_COUNT - 1] * esz[PT_COUNT - 1]; }
+  int put(const L& l, int k, const void* src, int r) {
+    CK(cudaMemcpyAsync(dst + off[k] + c0 * cols[k] * esz[k], src, (size_t)r * cols[k] * esz[k], cudaMemcpyDeviceToDevice, l.s));
+    return 0;
+  }
+};
+
+// decoder layer li over the r rows of one chunk at positions pos_base ..: residual x fp32 [r][H] updated in place, K/V into the pool;
+// a1 / a2 the chunk's operand buffers (see pf_bytes)
+static int prefill_layer(const L& l, int li, const int* page_row, long long pos_base, int r, float* x, bf16* a1, bf16* a2, PrefillTaps* taps) {
+  vv_ctx* c = l.c;
+  const auto& d = c->d;
   const int H = d.hidden_size, I = d.intermediate_size, nh = d.num_q_heads, nkv = d.num_kv_heads, hd = d.head_dim, nq = nh * hd;
   const int Nqkv = nq + 2 * nkv * hd;
-  unsigned char* ws = (unsigned char*)workspace;
-  float* x = (float*)ws;
-  bf16* a1 = (bf16*)(ws + align256(R * 4 * H));
-  bf16* a2 = (bf16*)(ws + align256(R * 4 * H) + align256(R * 2 * std::max(H, nq)));
   const size_t per_layer = (size_t)c->n_pages * nkv * KV_PAGE * hd;
-  const int* page_row = c->page_table_dev + (size_t)seq * c->max_pages;
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)hd);
-  L l{c, (cudaStream_t)stream};
   auto gemm = [&](auto kern, const bf16* A, const bf16* W, int M, int N, int K, PfGemm p) -> int {
     p.A = A; p.W = W; p.M = M; p.N = N; p.K = K;
     CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PF_SMEM));
     CK(launch_k(l, kern, dim3((N + PF_BN - 1) / PF_BN, (M + PF_BM - 1) / PF_BM), dim3(256), (size_t)PF_SMEM, p));
     return 0;
   };
+  const LmLayer& y = c->lm[li];
+  PfGemm p;
+  memset(&p, 0, sizeof p);
+  CK(launch_k(l, pf_rmsnorm_kernel, dim3((r + 7) / 8), dim3(256), 0, (const float*)x, (const float*)y.ln1, d.rms_norm_eps, r, H, a1));
+  if (taps) RET(taps->put(l, PT_NORM1, a1, r));
+  p.bias = y.bqkv; p.out = a2; p.ldo = nq; p.kpool = c->kpool + per_layer * li; p.vpool = c->vpool + per_layer * li; p.page_row = page_row;
+  p.nq = nq; p.kv_heads = nkv; p.pos_base = pos_base; p.inv_freq = c->inv_freq;
+  if (hd == 128) RET(gemm(pf_gemm_kernel<PF_EPI_QKV, 128>, a1, y.wqkv, r, Nqkv, H, p));
+  else RET(gemm(pf_gemm_kernel<PF_EPI_QKV, 64>, a1, y.wqkv, r, Nqkv, H, p));
+  if (taps) RET(taps->put(l, PT_Q, a2, r));
+  const dim3 ag((r + 63) / 64, nh);
+  if (hd == 128) {
+    CK(cudaFuncSetAttribute(pf_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PfAttnCfg<128>::SMEM));
+    CK(launch_k(l, pf_attn_kernel<128>, ag, dim3(128), (size_t)PfAttnCfg<128>::SMEM, (const bf16*)a2, r, nh, nkv, (const bf16*)p.kpool,
+                (const bf16*)p.vpool, page_row, pos_base, scale_log2, a1));
+  } else {
+    CK(cudaFuncSetAttribute(pf_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PfAttnCfg<64>::SMEM));
+    CK(launch_k(l, pf_attn_kernel<64>, ag, dim3(128), (size_t)PfAttnCfg<64>::SMEM, (const bf16*)a2, r, nh, nkv, (const bf16*)p.kpool,
+                (const bf16*)p.vpool, page_row, pos_base, scale_log2, a1));
+  }
+  if (taps) RET(taps->put(l, PT_ATTN, a1, r));
+  memset(&p, 0, sizeof p);
+  p.x = x; p.ldx = H;
+  RET(gemm(pf_gemm_kernel<PF_EPI_RESID>, a1, y.wo, r, H, nq, p));
+  if (taps) RET(taps->put(l, PT_RESID1, x, r));
+  CK(launch_k(l, pf_rmsnorm_kernel, dim3((r + 7) / 8), dim3(256), 0, (const float*)x, (const float*)y.ln2, d.rms_norm_eps, r, H, a1));
+  if (taps) RET(taps->put(l, PT_NORM2, a1, r));
+  memset(&p, 0, sizeof p);
+  p.out = a2; p.ldo = I;
+  RET(gemm(pf_gemm_kernel<PF_EPI_SWIGLU>, a1, y.wgu, r, 2 * I, H, p));
+  if (taps) RET(taps->put(l, PT_SWIGLU, a2, r));
+  memset(&p, 0, sizeof p);
+  p.x = x; p.ldx = H;
+  RET(gemm(pf_gemm_kernel<PF_EPI_RESID>, a2, y.wdown, r, H, I, p));
+  if (taps) RET(taps->put(l, PT_OUT, x, r));
+  return 0;
+}
+
+extern "C" int vv_lm_prefill(vv_ctx* c, int seq, int64_t pos0, int64_t n, const float* embeds, float* hidden_last, void* workspace,
+                             int64_t workspace_bytes, void* stream) {
+  RET(pf_check(c, n));
+  if (!embeds || !hidden_last || !workspace) return fail(VV_ERR_INVALID, "vv_lm_prefill: null argument");
+  if (((uintptr_t)embeds & 15) || ((uintptr_t)hidden_last & 15)) return fail(VV_ERR_INVALID, "vv_lm_prefill: embeds / hidden_last must be 16-byte aligned");
+  long long R;
+  RET(pf_begin(c, "vv_lm_prefill", seq, pos0, n, workspace, workspace_bytes, stream, &R));
+  const auto& d = c->d;
+  const int H = d.hidden_size, nq = d.num_q_heads * d.head_dim;
+  unsigned char* ws = (unsigned char*)workspace;
+  float* x = (float*)ws;
+  bf16* a1 = (bf16*)(ws + align256(R * 4 * H));
+  bf16* a2 = (bf16*)(ws + align256(R * 4 * H) + align256(R * 2 * std::max(H, nq)));
+  const int* page_row = c->page_table_dev + (size_t)seq * c->max_pages;
+  L l{c, (cudaStream_t)stream};
   for (long long c0 = 0; c0 < n; c0 += R) {
     const int r = (int)std::min<long long>(R, n - c0);
     CK(cudaMemcpyAsync(x, embeds + c0 * H, (size_t)r * H * 4, cudaMemcpyDeviceToDevice, l.s));
-    for (int li = 0; li < d.num_layers; ++li) {
-      const LmLayer& y = c->lm[li];
-      PfGemm p;
-      memset(&p, 0, sizeof p);
-      CK(launch_k(l, pf_rmsnorm_kernel, dim3((r + 7) / 8), dim3(256), 0, (const float*)x, (const float*)y.ln1, d.rms_norm_eps, r, H, a1));
-      p.bias = y.bqkv; p.out = a2; p.ldo = nq; p.kpool = c->kpool + per_layer * li; p.vpool = c->vpool + per_layer * li; p.page_row = page_row;
-      p.nq = nq; p.kv_heads = nkv; p.pos_base = pos0 + c0; p.inv_freq = c->inv_freq;
-      if (hd == 128) RET(gemm(pf_gemm_kernel<PF_EPI_QKV, 128>, a1, y.wqkv, r, Nqkv, H, p));
-      else RET(gemm(pf_gemm_kernel<PF_EPI_QKV, 64>, a1, y.wqkv, r, Nqkv, H, p));
-      const dim3 ag((r + 63) / 64, nh);
-      if (hd == 128) {
-        CK(cudaFuncSetAttribute(pf_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PfAttnCfg<128>::SMEM));
-        CK(launch_k(l, pf_attn_kernel<128>, ag, dim3(128), (size_t)PfAttnCfg<128>::SMEM, (const bf16*)a2, r, nh, nkv, (const bf16*)p.kpool,
-                    (const bf16*)p.vpool, page_row, (long long)(pos0 + c0), scale_log2, a1));
-      } else {
-        CK(cudaFuncSetAttribute(pf_attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PfAttnCfg<64>::SMEM));
-        CK(launch_k(l, pf_attn_kernel<64>, ag, dim3(128), (size_t)PfAttnCfg<64>::SMEM, (const bf16*)a2, r, nh, nkv, (const bf16*)p.kpool,
-                    (const bf16*)p.vpool, page_row, (long long)(pos0 + c0), scale_log2, a1));
-      }
-      memset(&p, 0, sizeof p);
-      p.x = x; p.ldx = H;
-      RET(gemm(pf_gemm_kernel<PF_EPI_RESID>, a1, y.wo, r, H, nq, p));
-      CK(launch_k(l, pf_rmsnorm_kernel, dim3((r + 7) / 8), dim3(256), 0, (const float*)x, (const float*)y.ln2, d.rms_norm_eps, r, H, a1));
-      memset(&p, 0, sizeof p);
-      p.out = a2; p.ldo = I;
-      RET(gemm(pf_gemm_kernel<PF_EPI_SWIGLU>, a1, y.wgu, r, 2 * I, H, p));
-      memset(&p, 0, sizeof p);
-      p.x = x; p.ldx = H;
-      RET(gemm(pf_gemm_kernel<PF_EPI_RESID>, a2, y.wdown, r, H, I, p));
-    }
+    for (int li = 0; li < d.num_layers; ++li) RET(prefill_layer(l, li, page_row, pos0 + c0, r, x, a1, a2, nullptr));
     if (c0 + r == n) CK(launch_k(l, rows_norm_block_kernel, dim3(1), dim3(256), 0, (const float*)(x + (size_t)(r - 1) * H), (const float*)c->lm_norm, hidden_last, H, d.rms_norm_eps));
   }
   return 0;
+}
+
+extern "C" int vv_debug_prefill_taps(vv_ctx* c, int seq, int64_t pos0, int64_t n, int layer, const float* x_in, float* hidden_last,
+                                     void* workspace, int64_t workspace_bytes, void* taps, int64_t taps_bytes, int32_t* meta, void* stream) {
+  RET(pf_check(c, n));
+  const auto& d = c->d;
+  if (layer < 0 || layer >= d.num_layers) return fail(VV_ERR_INVALID, "vv_debug_prefill_taps: bad layer %d", layer);
+  PrefillTaps sink(c, n);
+  if (meta)
+    for (int k = 0; k < PT_COUNT; ++k) { meta[3 * k] = k; meta[3 * k + 1] = sink.esz[k]; meta[3 * k + 2] = sink.cols[k]; }
+  if (!taps) return PT_COUNT;
+  if (taps_bytes < sink.bytes(n))
+    return fail(VV_ERR_INVALID, "vv_debug_prefill_taps: %lld bytes of tap space, the layer needs %lld", (long long)taps_bytes, sink.bytes(n));
+  if (!x_in || !workspace) return fail(VV_ERR_INVALID, "vv_debug_prefill_taps: null argument");
+  if (((uintptr_t)x_in & 15) || ((uintptr_t)hidden_last & 15)) return fail(VV_ERR_INVALID, "vv_debug_prefill_taps: x_in / hidden_last must be 16-byte aligned");
+  long long R;
+  RET(pf_begin(c, "vv_debug_prefill_taps", seq, pos0, n, workspace, workspace_bytes, stream, &R));
+  const int H = d.hidden_size, nq = d.num_q_heads * d.head_dim;
+  unsigned char* ws = (unsigned char*)workspace;
+  float* x = (float*)ws;
+  bf16* a1 = (bf16*)(ws + align256(R * 4 * H));
+  bf16* a2 = (bf16*)(ws + align256(R * 4 * H) + align256(R * 2 * std::max(H, nq)));
+  const int* page_row = c->page_table_dev + (size_t)seq * c->max_pages;
+  L l{c, (cudaStream_t)stream};
+  sink.dst = (unsigned char*)taps;
+  for (long long c0 = 0; c0 < n; c0 += R) {
+    const int r = (int)std::min<long long>(R, n - c0);
+    CK(cudaMemcpyAsync(x, x_in + c0 * H, (size_t)r * H * 4, cudaMemcpyDeviceToDevice, l.s));
+    sink.c0 = c0;
+    RET(prefill_layer(l, layer, page_row, pos0 + c0, r, x, a1, a2, &sink));
+    if (hidden_last && c0 + r == n) CK(launch_k(l, rows_norm_block_kernel, dim3(1), dim3(256), 0, (const float*)(x + (size_t)(r - 1) * H), (const float*)c->lm_norm, hidden_last, H, d.rms_norm_eps));
+  }
+  CK(cudaStreamSynchronize(l.s));
+  return PT_COUNT;
 }
 
 extern "C" int vv_embed_gather(vv_ctx* c, const int32_t* ids_dev, int64_t n, float* out, void* stream) {

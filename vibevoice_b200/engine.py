@@ -197,6 +197,36 @@ class Engine:
         cur.wait_stream(self.stream)
         return out
 
+    def prefill_taps(self, seq: int, layer: int, x: torch.Tensor, pos0: int = 0, workspace_bytes: Optional[int] = None):
+        """Decoder layer `layer` of `lm_prefill` alone on the residual input x [n, H] at positions pos0..pos0+n of sequence `seq`, with each
+        kernel's output copied out (`vv_debug_prefill_taps`, tests).  K/V land in the pool as in `lm_prefill`; the default workspace is
+        `lm_prefill`'s.  Returns ([(meta, tap)], hidden_last): meta = (kind, bytes per element, cols), tap = [n, cols] bf16 / fp32 on the
+        device; hidden_last [H] = the final-norm hidden state of the last output row."""
+        n = int(x.shape[0])
+        need = self.lm_prefill_workspace_bytes(n)
+        ws = int(workspace_bytes) if workspace_bytes is not None else min(need * ((n + 63) // 64), max(need, 2 << 30))
+        P = lambda t: C.c_void_p(None if t is None else t.data_ptr())
+        call = lambda xin, hl, work, w, taps, tb, meta, s: self.lib.vv_debug_prefill_taps(self.h, int(seq), int(pos0), n, int(layer), xin, hl, work,
+                                                                                          w, taps, tb, meta, s)
+        k = N.check(call(None, None, None, 0, None, 0, None, None), "vv_debug_prefill_taps")
+        meta = np.zeros((k, 3), dtype=np.int32)
+        N.check(call(None, None, None, 0, None, 0, N.iptr(meta), None), "vv_debug_prefill_taps")
+        sizes = [n * int(b) * int(c) for _, b, c in meta.tolist()]
+        cur = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            e = x.to(self.device, torch.float32).contiguous()
+            hl = torch.empty(self.config.decoder_config.hidden_size, dtype=torch.float32, device=self.device)
+            work = torch.empty(max(ws, 1), dtype=torch.uint8, device=self.device)
+            taps = torch.empty(sum(sizes), dtype=torch.uint8, device=self.device)
+            N.check(call(P(e), P(hl), P(work), ws, P(taps), taps.numel(), None, self.s), "vv_debug_prefill_taps")
+        cur.wait_stream(self.stream)
+        out, off = [], 0
+        for m, sz in zip(meta.tolist(), sizes):
+            out.append((tuple(m), taps[off:off + sz].view(torch.bfloat16 if m[1] == 2 else torch.float32).view(n, m[2])))
+            off += sz
+        return out, hl
+
     def embed_gather(self, ids) -> torch.Tensor:
         """token ids (any count) -> embedding rows [n, H] fp32 on the device (`vv_embed_gather`)."""
         ids = torch.as_tensor(ids).reshape(-1)
