@@ -244,6 +244,17 @@ int vv_debug_sampler_taps(vv_ctx* ctx, const float* cond, const float* noise, fl
 int vv_debug_prefill_taps(vv_ctx* ctx, int seq, int64_t pos0, int64_t n, int layer, const float* x_in, float* hidden_last, void* workspace,
                           int64_t workspace_bytes, void* taps, int64_t taps_bytes, int32_t* meta, void* stream);
 
+/* vv_voice_encode with every stage boundary copied out: it runs the same kernels in the same order, with the same voice groups and GEMM
+ * row chunks for the given workspace.  Tap k is [n][T_k][C_k] fp32 (time-major) at float offset n * sum_{j<k} T_j * C_j of `taps`; a
+ * group of voices writes its rows at its first voice's offset, so the layout does not depend on the workspace.  meta (optional)
+ * [n_taps][5] = {kind, stage, index, T, C}, in run order: kind 0 (i, 0) = output of stage i's convolution, (n_stages, 0) = the head conv
+ * (the latent mean [F][vae_dim]); 1 (i, j) = the mixer half x + gamma * dwconv7(RMSNorm(x)) of block j of stage i; 2 (i, j) = the output
+ * of that block; 3 (n_stages, 0) = the connector's fc1 output [F][H] before its RMSNorm; 4 (n_stages, 0) = the embeddings [F][H] (also
+ * written to embeds_out).  taps == NULL: fills meta and returns n_taps, nothing launched.  Errors: those of vv_voice_encode, and too
+ * little tap space -> VV_ERR_INVALID, all with nothing launched.  Returns n_taps.  Synchronises. */
+int vv_debug_voice_taps(vv_ctx* ctx, const float* wavs, int n, int64_t T, const float* sigma, const float* eps, float* embeds_out,
+                        void* workspace, int64_t workspace_bytes, float* taps, int64_t taps_floats, int32_t* meta, void* stream);
+
 int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_out);
 /* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).
  * prologue: 0 none, 1 RMSNorm(pro_w, eps), 3 SwiGLU pairs (x is [M][2K]), 4 GELU, 6 SiLU; alpha_kind: 0 one, 2 gamma[n]. Synchronises. */

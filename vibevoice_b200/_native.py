@@ -87,6 +87,7 @@ SYMBOLS = {
     "vv_debug_codec_taps": (_I, [_P, _I, _P, _P, _P, _P, _L, _P, _P]),
     "vv_debug_sampler_taps": (_I, [_P, _P, _P, _F, _P, _P, _L, _P, _P]),
     "vv_debug_prefill_taps": (_I, [_P, _I, _L, _L, _I, _P, _P, _P, _L, _P, _L, _P, _P]),
+    "vv_debug_voice_taps": (_I, [_P, _P, _I, _L, _P, _P, _P, _P, _L, _P, _L, _P, _P]),
     "vv_debug_stream_gemv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _F, _I, _P, _I, _P]),
     "vv_debug_stream_gemv2": (_I, [_P, _P, _P, _P, _L, _P, _L, _I, _I, _I, _I, _P, _F, _P, _P, _L, _I, _P, _L, _I, _L, _P]),
     "vv_stream_diag": (_I, [_P, _P]),

@@ -2343,8 +2343,47 @@ static int voice_conv(const L& l, const ConvL& cv, const float* x, long long T_i
   return 0;
 }
 
-// Block1D over x [nv][T][C] (result back in *x; *y is the other activation buffer)
-static int voice_block(const L& l, const Block& b, float** x, float** y, float* inv, int nv, long long T, unsigned char* S, long long Sb) {
+// ---- stage taps of vv_voice_encode (vv_debug_voice_taps): every stage boundary, [n][T_k][C_k] per tap, back to back.  A group of voices
+// writes its rows at voice offset v0 of every tap, so the layout does not depend on the grouping.  Production runs with no sink.
+enum { VT_CONV = 0, VT_MIX = 1, VT_BLOCK = 2, VT_FC1 = 3, VT_EMBEDS = 4 };
+// kind, stage, index: VT_CONV (i, 0) = output of stage i's convolution (i = n_stages: the head conv, the latent mean); VT_MIX (i, j) =
+// x + gamma * dwconv7(RMSNorm(x)) of block j of stage i; VT_BLOCK (i, j) = output of that block; VT_FC1 / VT_EMBEDS (n_stages, 0) = the
+// connector's fc1 output before its RMSNorm / the embeddings
+static void voice_tap_plan(const vv_ctx* c, const VoicePlan& pl, std::vector<TapMeta>* plan) {
+  const VoiceEnc& v = c->venc;
+  const int ns = (int)v.stages.size();
+  plan->clear();
+  for (int i = 0; i < ns; ++i) {
+    plan->push_back({VT_CONV, i, 0, (int)pl.T[i], v.C[i]});
+    for (int j = 0; j < (int)v.stages[i].size(); ++j) {
+      plan->push_back({VT_MIX, i, j, (int)pl.T[i], v.C[i]});
+      plan->push_back({VT_BLOCK, i, j, (int)pl.T[i], v.C[i]});
+    }
+  }
+  plan->push_back({VT_CONV, ns, 0, (int)pl.F, c->d.acoustic_vae_dim});
+  plan->push_back({VT_FC1, ns, 0, (int)pl.F, c->d.hidden_size});
+  plan->push_back({VT_EMBEDS, ns, 0, (int)pl.F, c->d.hidden_size});
+}
+struct VoiceTapSink {
+  std::vector<TapMeta> plan;
+  std::vector<long long> off;   // float offset of tap k: n * sum_{j<k} T_j * C_j
+  float* dst = nullptr;         // device
+  long long v0 = 0;             // first voice of the group being run
+  size_t next = 0;              // the group's next tap
+  // rows [r0, r0 + r) of the group's tap `next` (rows counted from the group's first voice); done: the tap is complete
+  int put(const L& l, int kind, int stage, int index, const float* src, long long r0, long long r, bool done = true) {
+    if (next >= plan.size() || plan[next].kind != kind || plan[next].stage != stage || plan[next].index != index)
+      return fail(VV_ERR_STATE, "voice taps: tap %zu (kind %d, stage %d, index %d) is not the planned one", next, kind, stage, index);
+    const TapMeta& t = plan[next];
+    CK(cudaMemcpyAsync(dst + off[next] + (v0 * t.T + r0) * t.C, src, (size_t)(r * t.C) * sizeof(float), cudaMemcpyDeviceToDevice, l.s));
+    if (done) ++next;
+    return 0;
+  }
+};
+
+// Block1D over x [nv][T][C] (result back in *x; *y is the other activation buffer); block j of stage i
+static int voice_block(const L& l, const Block& b, float** x, float** y, float* inv, int nv, long long T, unsigned char* S, long long Sb,
+                       VoiceTapSink* taps, int i, int j) {
   const int C = b.C;
   const float eps = l.c->d.codec_eps;
   const long long M = nv * T;
@@ -2352,6 +2391,7 @@ static int voice_block(const L& l, const Block& b, float** x, float** y, float* 
   CK(launch_k(l, voice_dwconv_kernel, dim3(ew_grid(l.c, M * C)), dim3(256), 0, (const float*)*x, (const float*)inv, (const float*)b.norm_w,
               (const float*)b.dw_w, (const float*)b.dw_b, (const float*)b.gamma, *y, M, (int)T, C));
   std::swap(*x, *y);
+  if (taps) RET(taps->put(l, VT_MIX, i, j, *x, 0, M));
   // FFN in row chunks (no halo): norm -> planes -> C x 4C GEMM + GELU -> planes -> 4C x C GEMM, gamma residual in place
   const long long R = voice_chunk(Sb, 32ll * C, M);
   float* hid = (float*)S;
@@ -2366,19 +2406,20 @@ static int voice_block(const L& l, const Block& b, float** x, float** y, float* 
                 (int)r, 4 * C));
     RET(voice_gemm(l, b.w2, b.b2, C, 4 * C, planes, planes + r * 4 * C, r, xr, C, EPI_GAMMA_RESID, b.ffn_gamma));
   }
+  if (taps) RET(taps->put(l, VT_BLOCK, i, j, *x, 0, M));
   return 0;
 }
 
-extern "C" int vv_voice_encode(vv_ctx* c, const float* wavs, int n, int64_t T, const float* sigma, const float* eps, float* mean_out,
-                               float* embeds_out, void* workspace, int64_t workspace_bytes, void* stream) {
-  RET(voice_check(c, n, T));
-  if (!wavs || !embeds_out || !workspace || (eps && !sigma)) return fail(VV_ERR_INVALID, "vv_voice_encode: null argument");
-  if (((uintptr_t)workspace & 255) || ((uintptr_t)eps & 15)) return fail(VV_ERR_INVALID, "vv_voice_encode: workspace must be 256-byte and eps 16-byte aligned");
+// what vv_voice_encode runs, with every stage boundary copied into `taps` when it is given
+static int voice_run(vv_ctx* c, const char* who, const float* wavs, int n, int64_t T, const float* sigma, const float* eps, float* mean_out,
+                     float* embeds_out, void* workspace, int64_t workspace_bytes, void* stream, VoiceTapSink* taps) {
+  if (!wavs || !embeds_out || !workspace || (eps && !sigma)) return fail(VV_ERR_INVALID, "%s: null argument", who);
+  if (((uintptr_t)workspace & 255) || ((uintptr_t)eps & 15)) return fail(VV_ERR_INVALID, "%s: workspace must be 256-byte and eps 16-byte aligned", who);
   VoicePlan pl;
   voice_plan(c, T, &pl);
   const long long smin = voice_scratch_min(pl), need = voice_act_bytes(c, pl, 1) + smin;
   if (workspace_bytes < need)
-    return fail(VV_ERR_INVALID, "vv_voice_encode: workspace of %lld bytes is below the minimum %lld", (long long)workspace_bytes, need);
+    return fail(VV_ERR_INVALID, "%s: workspace of %lld bytes is below the minimum %lld", who, (long long)workspace_bytes, need);
   long long g = n;
   while (g > 1 && voice_act_bytes(c, pl, g) + smin > workspace_bytes) --g;
   CK(cudaSetDevice(c->device));
@@ -2396,13 +2437,16 @@ extern "C" int vv_voice_encode(vv_ctx* c, const float* wavs, int n, int64_t T, c
   L l{c, (cudaStream_t)stream};
   for (long long v0 = 0; v0 < n; v0 += g) {
     const int nv = (int)std::min<long long>(g, n - v0);
+    if (taps) { taps->v0 = v0; taps->next = 0; }
     float *x = bufA, *y = bufB;
     for (int i = 0; i < ns; ++i) {
       if (i == 0) RET(voice_conv(l, v.convs[0], wavs + v0 * T, T, T, nv, x, S, Sb));
       else { RET(voice_conv(l, v.convs[i], x, pl.T[i - 1], pl.T[i], nv, y, S, Sb)); std::swap(x, y); }
-      for (const Block& b : v.stages[i]) RET(voice_block(l, b, &x, &y, inv, nv, pl.T[i], S, Sb));
+      if (taps) RET(taps->put(l, VT_CONV, i, 0, x, 0, nv * pl.T[i]));
+      for (int j = 0; j < (int)v.stages[i].size(); ++j) RET(voice_block(l, v.stages[i][j], &x, &y, inv, nv, pl.T[i], S, Sb, taps, i, j));
     }
     RET(voice_conv(l, v.convs[ns], x, F, F, nv, mean, S, Sb));
+    if (taps) RET(taps->put(l, VT_CONV, ns, 0, mean, 0, nv * F));
     if (mean_out) CK(cudaMemcpyAsync(mean_out + v0 * F * D, mean, (size_t)nv * F * D * 4, cudaMemcpyDeviceToDevice, l.s));
     // x = mean + sigma * eps; feat = (x + bias) * scale; acoustic_connector = fc2(RMSNorm_1e-6(fc1(feat)))
     const long long M = nv * F, R = voice_chunk(Sb, 8ll * H, M);
@@ -2413,12 +2457,47 @@ extern "C" int vv_voice_encode(vv_ctx* c, const float* wavs, int n, int64_t T, c
       CK(launch_k(l, voice_sample_split_kernel, dim3(ew_grid(c, r * D / 4)), dim3(256), 0, (const float*)mean, eps ? eps + v0 * F * D : nullptr,
                   sigma ? sigma + v0 : nullptr, (int)F, D, c->speech_bias, c->speech_scale, m0, (int)r, planes, planes + r * D));
       RET(voice_gemm(l, c->ca_fc1, c->ca_b1, H, D, planes, planes + r * D, r, y1, H));
+      if (taps) RET(taps->put(l, VT_FC1, ns, 0, y1, m0, r, m0 + r == M));
       CK(launch_k(l, voice_norm_split_kernel, dim3((unsigned)((r + 7) / 8)), dim3(256), 0, (const float*)y1, (const float*)c->ca_n, 1e-6f, (int)r, H,
                   planes, planes + r * H));
       RET(voice_gemm(l, c->ca_fc2, c->ca_b2, H, H, planes, planes + r * H, r, embeds_out + (v0 * F + m0) * H, H));
     }
+    if (taps) {
+      RET(taps->put(l, VT_EMBEDS, ns, 0, embeds_out + v0 * F * H, 0, M));
+      if (taps->next != taps->plan.size()) return fail(VV_ERR_STATE, "%s: a group made %zu of %zu taps", who, taps->next, taps->plan.size());
+    }
   }
   return 0;
+}
+
+extern "C" int vv_voice_encode(vv_ctx* c, const float* wavs, int n, int64_t T, const float* sigma, const float* eps, float* mean_out,
+                               float* embeds_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  RET(voice_check(c, n, T));
+  return voice_run(c, "vv_voice_encode", wavs, n, T, sigma, eps, mean_out, embeds_out, workspace, workspace_bytes, stream, nullptr);
+}
+
+extern "C" int vv_debug_voice_taps(vv_ctx* c, const float* wavs, int n, int64_t T, const float* sigma, const float* eps, float* embeds_out,
+                                   void* workspace, int64_t workspace_bytes, float* taps, int64_t taps_floats, int32_t* meta, void* stream) {
+  RET(voice_check(c, n, T));
+  VoicePlan pl;
+  voice_plan(c, T, &pl);
+  VoiceTapSink sink;
+  voice_tap_plan(c, pl, &sink.plan);
+  const int nt = (int)sink.plan.size();
+  long long need = 0;
+  for (int k = 0; k < nt; ++k) {
+    const TapMeta& t = sink.plan[k];
+    sink.off.push_back(need);
+    need += (long long)n * t.T * t.C;
+    if (meta) { int32_t* m = meta + 5 * k; m[0] = t.kind; m[1] = t.stage; m[2] = t.index; m[3] = t.T; m[4] = t.C; }
+  }
+  if (!taps) return nt;
+  if (taps_floats < need)
+    return fail(VV_ERR_INVALID, "vv_debug_voice_taps: %lld floats of tap space, the encoder needs %lld", (long long)taps_floats, need);
+  sink.dst = taps;
+  RET(voice_run(c, "vv_debug_voice_taps", wavs, n, T, sigma, eps, nullptr, embeds_out, workspace, workspace_bytes, stream, &sink));
+  CK(cudaStreamSynchronize((cudaStream_t)stream));
+  return nt;
 }
 
 // ------------------------------------------------------------------------------------------------

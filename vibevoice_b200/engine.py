@@ -174,6 +174,37 @@ class Engine:
         cur.wait_stream(self.stream)
         return out
 
+    def voice_taps(self, wavs: torch.Tensor, sigma: torch.Tensor, eps: Optional[torch.Tensor], workspace_bytes: Optional[int] = None):
+        """`voice_encode` with every stage boundary copied out (`vv_debug_voice_taps`, tests), on `voice_encode`'s default workspace unless
+        one is given.  Returns ([(meta, tap)], embeds): meta = (kind, stage, index, T, C), tap = [n, T, C] fp32 on the device (a 10 s voice
+        at full width has about 0.8 GB of taps); embeds [n, F, H]."""
+        n, T = wavs.shape
+        need = self.voice_workspace_bytes(n, T)
+        ws = int(workspace_bytes) if workspace_bytes is not None else min(need * n + (256 << 20), max(need, 2 << 30))
+        F, H = self.voice_frames(T), self.config.decoder_config.hidden_size
+        P = lambda t: C.c_void_p(None if t is None else t.data_ptr())
+        call = lambda w, s, e, out, work, taps, nt, meta, st: self.lib.vv_debug_voice_taps(self.h, w, n, T, s, e, out, work, ws, taps, nt, meta, st)
+        k = N.check(call(None, None, None, None, None, None, 0, None, None), "vv_debug_voice_taps")
+        meta = np.zeros((k, 5), dtype=np.int32)
+        N.check(call(None, None, None, None, None, None, 0, N.iptr(meta), None), "vv_debug_voice_taps")
+        sizes = [n * int(t) * int(c) for t, c in meta[:, 3:]]
+        cur = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            wavs = wavs.to(self.device, torch.float32).contiguous()
+            sigma = sigma.to(self.device, torch.float32).contiguous()
+            eps = None if eps is None else eps.to(self.device, torch.float32).contiguous()
+            out = torch.empty(n, F, H, dtype=torch.float32, device=self.device)
+            work = torch.empty(max(ws, 1), dtype=torch.uint8, device=self.device)
+            taps = torch.empty(sum(sizes), dtype=torch.float32, device=self.device)
+            N.check(call(P(wavs), P(sigma), P(eps), P(out), P(work), P(taps), taps.numel(), None, self.s), "vv_debug_voice_taps")
+        cur.wait_stream(self.stream)
+        res, off = [], 0
+        for m, sz in zip(meta.tolist(), sizes):
+            res.append((tuple(m), taps[off:off + sz].view(n, m[3], m[4])))
+            off += sz
+        return res, out
+
     # ---- f-2 native prompt prefill ---------------------------------------------------------------------
     def lm_prefill_workspace_bytes(self, n_tokens: int) -> int:
         """minimum workspace of `lm_prefill` (one 64-row chunk)."""
