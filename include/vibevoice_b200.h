@@ -87,7 +87,8 @@ void vv_destroy(vv_ctx* ctx);
 int vv_load_tensor(vv_ctx* ctx, const char* name, const void* data, int dtype, const int64_t* shape, int ndim);
 int vv_set_speech_factors(vv_ctx* ctx, float scaling_factor, float bias_factor); /* modeling_vibevoice.py:131-132 */
 int vv_finalize_weights(vv_ctx* ctx);     /* fails with the list of missing tensors */
-int64_t vv_weight_bytes(vv_ctx* ctx, int which); /* 0 lm, 1 head-per-step, 2 cond_proj, 3 decoder, 4 semantic, 5 connectors */
+int64_t vv_weight_bytes(vv_ctx* ctx, int which); /* 0 lm, 1 head-per-step, 2 cond_proj, 3 decoder, 4 semantic, 5 connectors,
+                                                    6 streaming heads (0 when the checkpoint has none) */
 
 /* ---- paged KV cache (replaces HF DynamicCache, modeling_vibevoice_inference.py:303, 556-562) -- *
  * 2B sequences share one pool of pages (64 tokens each, all layers); pages return to the pool when vv_kv_set_len shrinks a sequence. */
@@ -187,6 +188,18 @@ int vv_lm_prefill(vv_ctx* ctx, int seq, int64_t pos0, int64_t n_tokens, const fl
 /* embedding rows of DEVICE token ids (any count; vv_embed_tokens takes at most 16 host ids): out [n,H] fp32; ids outside [0, vocab) give
  * zero rows. */
 int vv_embed_gather(vv_ctx* ctx, const int32_t* ids_dev, int64_t n, float* out, void* stream);
+
+/* ---- streaming-0.5B per-token modules (modeling_vibevoice_streaming.py:42-53, 124-131) ------------------------------------------ *
+ * Optional weights: model.tts_input_types.weight [2,H], tts_eos_classifier.fc1.{weight [H,H], bias [H]}, fc2.{weight [1,H], bias [1]},
+ * all five or none (else vv_finalize_weights fails), kept in fp32 whatever dtype they arrive in; without them both calls return
+ * VV_ERR_STATE and vv_weight_bytes(ctx, 6) is 0.
+ * vv_tts_type_embed: dst[rows[i]] = src + tts_input_types[type_id] for i < n (n <= 16 host row indices, rows of H fp32 floats; src may be
+ * one of them).  One fp32 add per element.
+ * vv_eos_prob: prob_out[0] = sigmoid(fc2 . relu(fc1 . hidden + b1) + b2), logit_out[0] (may be NULL) = the logit; hidden [H] fp32, all
+ * device pointers.  One launch, fp32 accumulation in a fixed order (results are bit-identical from call to call); calls on one ctx must
+ * not overlap (they share a workspace). */
+int vv_tts_type_embed(vv_ctx* ctx, const float* src, int type_id, const int32_t* rows_host, int n, float* dst, void* stream);
+int vv_eos_prob(vv_ctx* ctx, const float* hidden, float* prob_out, float* logit_out, void* stream);
 
 /* ---- introspection for tests / bench ----------------------------------------------------------- */
 /* the inverse of vv_kv_write: K / V [n][kv_heads][head_dim] bf16 of positions [pos0, pos0 + n) of (seq, layer); either output may be NULL */

@@ -1,1 +1,1 @@
-from vibevoice_b200.processor import VibeVoiceProcessor  # noqa: F401
+from vibevoice_b200.processor import VibeVoiceProcessor, VibeVoiceStreamingProcessor  # noqa: F401

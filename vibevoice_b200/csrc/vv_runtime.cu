@@ -9,6 +9,7 @@
 #include "vv_stream.cuh"
 #include "vv_voice.cuh"
 #include "vv_prefill.cuh"
+#include "vv_tts.cuh"
 
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -104,6 +105,7 @@ struct vv_ctx {
   std::map<std::string, RawTensor> raw;
   std::set<std::string> expected;
   std::set<std::string> voice_expected;      // acoustic encoder tensors: all or none
+  std::set<std::string> tts_expected;        // streaming-0.5B type embeddings + EOS classifier: all or none
   std::vector<void*> allocs;
   float speech_scale = NAN, speech_bias = NAN;
   // LM
@@ -122,7 +124,10 @@ struct vv_ctx {
   float *ca_b1 = nullptr, *ca_b2 = nullptr, *ca_n = nullptr, *cs_b1 = nullptr, *cs_b2 = nullptr, *cs_n = nullptr;
   Codec dec, enc;
   VoiceEnc venc;
-  int64_t wbytes[6] = {0, 0, 0, 0, 0, 0};
+  int64_t wbytes[7] = {0, 0, 0, 0, 0, 0, 0};
+  // streaming-0.5B per-token modules (vv_tts.cuh); present iff the checkpoint has them
+  float *tts_types = nullptr, *eos_w1 = nullptr, *eos_b1 = nullptr, *eos_w2 = nullptr, *eos_b2 = nullptr;
+  float* eos_partial = nullptr; unsigned* eos_ticket = nullptr;
   // KV
   int64_t n_pages = 0; int max_pages = 0; bf16 *kpool = nullptr, *vpool = nullptr;
   int* page_table_dev = nullptr; int* kv_len_dev = nullptr; int* row_mode_dev = nullptr;
@@ -672,6 +677,9 @@ static void build_expected(vv_ctx* c) {
     for (int j = 0; j < d.enc_depths[i]; ++j) block_names(v, S("%s.stages.%d.%d", ap.c_str(), i, j));
   }
   for (const char* s : {"head.conv.conv.weight", "head.conv.conv.bias"}) v.insert(ap + "." + s);
+  for (const char* s : {"model.tts_input_types.weight", "tts_eos_classifier.fc1.weight", "tts_eos_classifier.fc1.bias",
+                        "tts_eos_classifier.fc2.weight", "tts_eos_classifier.fc2.bias"})
+    c->tts_expected.insert(s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -722,6 +730,7 @@ extern "C" void vv_destroy(vv_ctx* c) {
 
 static bool stored_as_f32(const std::string& name, const int64_t* shape, int ndim) {
   if (ndim <= 1) return true;
+  if (name.rfind("model.tts_input_types.", 0) == 0 || name.rfind("tts_eos_classifier.", 0) == 0) return true;   // kept exact (vv_tts.cuh)
   if (name.find("mixer.conv.conv.conv.weight") != std::string::npos) return true;                 // depthwise [C,1,7]
   if (ndim == 3 && (shape[0] == 1 || shape[1] == 1)) return true;                                  // 1->32 stem, 32->1 head
   return false;
@@ -741,7 +750,7 @@ extern "C" int vv_load_tensor(vv_ctx* c, const char* name_, const void* data, in
     (name == "model.speech_scaling_factor" ? c->speech_scale : c->speech_bias) = v;
     return 0;
   }
-  if (!c->expected.count(name) && !c->voice_expected.count(name)) {
+  if (!c->expected.count(name) && !c->voice_expected.count(name) && !c->tts_expected.count(name)) {
     if (name.find("fix_std") != std::string::npos ||
         name.find("rotary_emb") != std::string::npos || (name == "lm_head.weight" && c->d.tie_word_embeddings))
       return 1;   // not on this path
@@ -937,6 +946,25 @@ static int build_voice_encoder(vv_ctx* c) {
   }
   RET(build_conv_gemm(c, p + ".head.conv.conv", nf << (ns - 1), d.acoustic_vae_dim, 7, 1, &v.convs[ns], &v.weight_bytes));
   v.present = true;
+  return 0;
+}
+
+// streaming-0.5B type embeddings and EOS classifier for vv_tts_type_embed / vv_eos_prob: packed iff the checkpoint has them, all of them
+static int build_tts_heads(vv_ctx* c) {
+  int nm = 0;
+  for (auto& n : c->tts_expected) nm += !c->raw.count(n);
+  if (nm == (int)c->tts_expected.size()) return 0;
+  if (nm) return fail(VV_ERR_STATE, "streaming heads: %d of %zu tensors (model.tts_input_types, tts_eos_classifier) missing", nm,
+                      c->tts_expected.size());
+  const int H = c->d.hidden_size;
+  int64_t* b = &c->wbytes[6];
+  RET(take_f32(c, "model.tts_input_types.weight", {2, H}, &c->tts_types, b));
+  RET(take_f32(c, "tts_eos_classifier.fc1.weight", {H, H}, &c->eos_w1, b));
+  RET(take_f32(c, "tts_eos_classifier.fc1.bias", {H}, &c->eos_b1, b));
+  RET(take_f32(c, "tts_eos_classifier.fc2.weight", {1, H}, &c->eos_w2, b));
+  RET(take_f32(c, "tts_eos_classifier.fc2.bias", {1}, &c->eos_b2, b));
+  RET(dmalloc(c, &c->eos_partial, (size_t)(H + EOS_ROWS_PER_CTA - 1) / EOS_ROWS_PER_CTA));
+  RET(dmalloc(c, &c->eos_ticket, 1));
   return 0;
 }
 
@@ -1172,6 +1200,7 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     k.weight_bytes = *kb;
   }
   RET(build_voice_encoder(c));
+  RET(build_tts_heads(c));
   max_win = std::max(max_win, (size_t)(hop + 8) * 64);
   RET(dmalloc(c, &c->s_xa, (size_t)B * max_tc));
   RET(dmalloc(c, &c->s_xb, (size_t)B * max_tc));
@@ -1205,7 +1234,7 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
   return 0;
 }
 
-extern "C" int64_t vv_weight_bytes(vv_ctx* c, int which) { return (c && which >= 0 && which < 6) ? c->wbytes[which] : -1; }
+extern "C" int64_t vv_weight_bytes(vv_ctx* c, int which) { return (c && which >= 0 && which < 7) ? c->wbytes[which] : -1; }
 extern "C" int64_t vv_launch_count(vv_ctx* c) { return c ? c->launches : -1; }
 
 // ------------------------------------------------------------------------------------------------
@@ -2695,6 +2724,37 @@ extern "C" int vv_embed_gather(vv_ctx* c, const int32_t* ids_dev, int64_t n, flo
                                                                                                    c->d.hidden_size, out);
   CKL();
   c->launches++;
+  return 0;
+}
+
+extern "C" int vv_tts_type_embed(vv_ctx* c, const float* src, int type_id, const int32_t* rows_host, int n, float* dst, void* stream) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->tts_types) return fail(VV_ERR_STATE, "vv_tts_type_embed: no model.tts_input_types loaded");
+  if (!src || !dst || !rows_host) return fail(VV_ERR_INVALID, "vv_tts_type_embed: null argument");
+  if (type_id < 0 || type_id > 1) return fail(VV_ERR_INVALID, "vv_tts_type_embed: type_id %d not 0 or 1", type_id);
+  if (n < 1 || n > TTS_MAX_ROWS) return fail(VV_ERR_INVALID, "vv_tts_type_embed: n = %d rows (1..%d)", n, TTS_MAX_ROWS);
+  TtsRows rows;
+  rows.n = n;
+  for (int i = 0; i < n; ++i) {
+    if (rows_host[i] < 0) return fail(VV_ERR_INVALID, "vv_tts_type_embed: negative row %d", rows_host[i]);
+    rows.row[i] = rows_host[i];
+  }
+  CK(cudaSetDevice(c->device));
+  const int H = c->d.hidden_size;
+  CK(launch_k(L{c, (cudaStream_t)stream}, tts_type_embed_kernel, dim3((H + 255) / 256), dim3(256), 0, src, (const float*)c->tts_types,
+              type_id, rows, dst, H));
+  return 0;
+}
+
+extern "C" int vv_eos_prob(vv_ctx* c, const float* hidden, float* prob_out, float* logit_out, void* stream) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->eos_w1) return fail(VV_ERR_STATE, "vv_eos_prob: no tts_eos_classifier loaded");
+  if (!hidden || !prob_out) return fail(VV_ERR_INVALID, "vv_eos_prob: null argument");
+  CK(cudaSetDevice(c->device));
+  const int H = c->d.hidden_size;
+  CK(launch_k(L{c, (cudaStream_t)stream}, eos_prob_kernel, dim3((H + EOS_ROWS_PER_CTA - 1) / EOS_ROWS_PER_CTA), dim3(EOS_THREADS),
+              (size_t)H * sizeof(float), hidden, (const float*)c->eos_w1, (const float*)c->eos_b1, (const float*)c->eos_w2,
+              (const float*)c->eos_b2, H, c->eos_partial, c->eos_ticket, prob_out, logit_out));
   return 0;
 }
 

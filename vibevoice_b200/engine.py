@@ -87,6 +87,8 @@ class Engine:
         self.logits_h = torch.zeros(B, len(self.valid_ids), dtype=torch.float32).pin_memory()
         self.noise_h = torch.zeros(B, 64, dtype=torch.float32).pin_memory()
         self.active_h = torch.zeros(B, dtype=torch.int32).pin_memory()
+        self.eos_d = torch.zeros(2, dtype=torch.float32, device=dev)       # vv_eos_prob: probability, logit
+        self.eos_h = torch.zeros(2, dtype=torch.float32).pin_memory()
         self.n_steps = 0
         self.step_noise = None
         self.scheduler = DPMSolverMultistepScheduler(
@@ -283,6 +285,44 @@ class Engine:
                                               self.s), "vv_debug_kv_read")
         self.stream.synchronize()
         return k, v
+
+    # ---- streaming-0.5B type embeddings and EOS classifier (csrc/vv_tts.cuh) ------------------------------
+    @property
+    def has_tts_heads(self) -> bool:
+        """whether the loaded checkpoint carried `model.tts_input_types` and `tts_eos_classifier` (known after finalize)."""
+        return int(self.lib.vv_weight_bytes(self.h, 6)) > 0
+
+    def _row_of(self, t: torch.Tensor, what: str):
+        H = self.config.decoder_config.hidden_size
+        if t.device != self.device or t.dtype != torch.float32 or t.shape[-1] != H or t.stride(-1) != 1:
+            raise ValueError("%s must be fp32 rows of %d contiguous floats on %s" % (what, H, self.device))
+
+    def tts_type_embed(self, src: torch.Tensor, type_id: int, rows, dst: torch.Tensor):
+        """`dst[r] = src + tts_input_types[type_id]` for r in `rows` on the engine stream (1 = text, 0 = speech), which must see src
+        complete, like every engine call.  src [H] may be a row of dst [R, H]."""
+        self._row_of(src, "src")
+        self._row_of(dst, "dst")
+        if src.dim() != 1 or dst.dim() != 2 or not dst.is_contiguous():
+            raise ValueError("src must be [H] and dst a contiguous [R, H]")
+        if any(not 0 <= int(r) < dst.shape[0] for r in rows):
+            raise ValueError("rows %s outside dst's %d rows" % (list(rows), dst.shape[0]))
+        r = N.i32(rows)
+        N.check(self.lib.vv_tts_type_embed(self.h, C.c_void_p(src.data_ptr()), int(type_id), N.iptr(r), len(r), C.c_void_p(dst.data_ptr()),
+                                           self.s), "vv_tts_type_embed")
+
+    def eos_prob(self, hidden: Optional[torch.Tensor] = None) -> float:
+        """`sigmoid(tts_eos_classifier(hidden))` (default: hidden row 0), synchronising the engine stream; `eos_logit` keeps the logit."""
+        h = self.hidden[0] if hidden is None else hidden
+        self._row_of(h, "hidden")
+        if h.dim() != 1:
+            raise ValueError("hidden must be [H]")
+        N.check(self.lib.vv_eos_prob(self.h, C.c_void_p(h.data_ptr()), C.c_void_p(self.eos_d.data_ptr()),
+                                     C.c_void_p(self.eos_d.data_ptr() + 4), self.s), "vv_eos_prob")
+        with torch.cuda.stream(self.stream):
+            self.eos_h.copy_(self.eos_d, non_blocking=True)
+        self.stream.synchronize()
+        self.eos_logit = float(self.eos_h[1])
+        return float(self.eos_h[0])
 
     # ---- KV -----------------------------------------------------------------------------------------
     def kv_init(self, total_tokens: int):

@@ -1,4 +1,5 @@
-"""`VibeVoiceProcessor` -- script + voice samples -> model inputs, and `save_audio`.
+"""`VibeVoiceProcessor` -- script + voice samples -> model inputs, and `save_audio`; `VibeVoiceStreamingProcessor` -- text + a cached
+voice prompt -> the streaming-0.5B model's inputs.
 
 Same call surface and output keys as the reference (`vibevoice/processor/vibevoice_processor.py:163-244, 374-404, 677-696`):
 `input_ids, attention_mask, speech_input_mask, speech_tensors, speech_masks, parsed_scripts, all_speakers_list`, left-padded
@@ -84,6 +85,14 @@ def convert_to_16_bit_wav(data) -> np.ndarray:
     return (data * 32767).astype(np.int16)
 
 
+def _set_speech_token_ids(tokenizer):
+    """The special-token ids the VibeVoice tokenizers expose as attributes (`modular_vibevoice_text_tokenizer.py:163-181`)."""
+    ids = tokenizer.convert_tokens_to_ids
+    tokenizer.speech_start_id, tokenizer.speech_end_id = ids("<|vision_start|>"), ids("<|vision_end|>")
+    tokenizer.speech_diffusion_id, tokenizer.pad_id = ids("<|vision_pad|>"), ids("<|image_pad|>")
+    return tokenizer
+
+
 class VibeVoiceProcessor:
     def __init__(self, tokenizer=None, audio_processor=None, speech_tok_compress_ratio: int = 3200, db_normalize: bool = True, **kwargs):
         self.tokenizer = tokenizer
@@ -103,10 +112,7 @@ class VibeVoiceProcessor:
         if tokenizer is None:
             try:   # a Qwen2.5 tokenizer next to the checkpoint (the reference resolves `language_model_pretrained_name` on the hub)
                 from transformers import AutoTokenizer
-                tokenizer = AutoTokenizer.from_pretrained(path)
-                ids = tokenizer.convert_tokens_to_ids
-                tokenizer.speech_start_id, tokenizer.speech_end_id = ids("<|vision_start|>"), ids("<|vision_end|>")
-                tokenizer.speech_diffusion_id, tokenizer.pad_id = ids("<|vision_pad|>"), ids("<|image_pad|>")
+                tokenizer = _set_speech_token_ids(AutoTokenizer.from_pretrained(path))
             except Exception as e:
                 raise FileNotFoundError("no tokenizer files under %s (offline image): pass tokenizer=... explicitly" % path) from e
         return cls(tokenizer=tokenizer, speech_tok_compress_ratio=cfg.get("speech_tok_compress_ratio", 3200),
@@ -300,3 +306,86 @@ class VibeVoiceProcessor:
 
     def decode(self, *a, **k):
         return self.tokenizer.decode(*a, **k)
+
+
+class VibeVoiceStreamingProcessor:
+    """Inputs of the streaming-0.5B model (`VibeVoiceStreamingForConditionalGenerationInference.generate`) from one text and a cached
+    voice prompt: the `all_prefilled_outputs` dict of a shipped preset (`demo/voices/streaming_model/*.pt`), whose four model outputs
+    already hold the voice's K/V.  Same surface and output keys as the reference's `vibevoice/processor/vibevoice_streaming_processor.py`;
+    the prompt positions are represented by `tokenizer.pad_id` placeholders, one per cached position of each stack."""
+
+    def __init__(self, tokenizer=None, audio_processor=None, speech_tok_compress_ratio: int = 3200, db_normalize: bool = True, **kwargs):
+        self.tokenizer = tokenizer
+        self.audio_processor = audio_processor
+        self.speech_tok_compress_ratio = speech_tok_compress_ratio
+        self.db_normalize = db_normalize
+        self.audio_normalizer = AudioNormalizer() if db_normalize else None
+        self.sampling_rate = 24000
+
+    @classmethod
+    def from_pretrained(cls, path: str, tokenizer=None, **kwargs):
+        """`path/preprocessor_config.json` (defaults when absent).  The tokenizer is, in order: `tokenizer=`; tokenizer files in `path`;
+        `language_model_pretrained_name` (config, else keyword) from the local Hugging Face cache only.  Nothing is downloaded."""
+        cfg = {}
+        f = os.path.join(path, "preprocessor_config.json")
+        if os.path.exists(f):
+            with open(f) as fh:
+                cfg = json.load(fh)
+        if tokenizer is None:
+            from transformers import AutoTokenizer
+            name = cfg.get("language_model_pretrained_name") or kwargs.get("language_model_pretrained_name")
+            errors = []
+            for src in ([path] if os.path.isdir(path) else []) + ([name] if name else []):
+                try:
+                    tokenizer = _set_speech_token_ids(AutoTokenizer.from_pretrained(src, local_files_only=True))
+                    break
+                except Exception as e:   # no tokenizer files there / not in the local cache
+                    errors.append("%s: %s" % (src, e))
+            if tokenizer is None:
+                raise FileNotFoundError("no tokenizer found offline for %s (tried %s): pass tokenizer=... explicitly"
+                                        % (path, "; ".join(errors) or "nothing"))
+        return cls(tokenizer=tokenizer, speech_tok_compress_ratio=cfg.get("speech_tok_compress_ratio", 3200),
+                   db_normalize=cfg.get("db_normalize", True))
+
+    def save_pretrained(self, save_directory: str, **kwargs):
+        """Writes `preprocessor_config.json` in the reference's format (what `from_pretrained` reads back)."""
+        os.makedirs(save_directory, exist_ok=True)
+        ap = self.audio_processor
+        cfg = {"processor_class": "VibeVoiceStreamingProcessor", "speech_tok_compress_ratio": self.speech_tok_compress_ratio,
+               "db_normalize": self.db_normalize,
+               "audio_processor": {"feature_extractor_type": "VibeVoiceTokenizerProcessor",
+                                   "sampling_rate": getattr(ap, "sampling_rate", self.sampling_rate),
+                                   "normalize_audio": getattr(ap, "normalize_audio", True),
+                                   "target_dB_FS": getattr(ap, "target_dB_FS", -25), "eps": getattr(ap, "eps", 1e-6)}}
+        with open(os.path.join(save_directory, "preprocessor_config.json"), "w") as fh:
+            json.dump(cfg, fh, indent=2)
+
+    def __call__(self, *args, **kwargs):
+        raise NotImplementedError("VibeVoiceStreamingProcessor.__call__ is not implemented. "
+                                  "Use process_input_with_cached_prompt for streaming inputs.")
+
+    def process_input_with_cached_prompt(self, text: Optional[str] = None, cached_prompt: Optional[Dict[str, Any]] = None, padding=True,
+                                         truncation=False, max_length: Optional[int] = None, return_tensors=None,
+                                         return_attention_mask: bool = True, **kwargs) -> BatchEncoding:
+        """One text and its cached prompt -> `input_ids` / `tts_lm_input_ids` (`pad_id` placeholders as long as the prompt's `lm` /
+        `tts_lm` outputs), `tts_text_ids` = `encode(text.strip() + "\\n")` without special tokens, the two attention masks (all ones),
+        `speech_input_mask` (all False) and `speech_tensors = speech_masks = None`.  A batch of one: `padding`, `truncation` and
+        `max_length` have nothing to act on."""
+        tok = self.tokenizer
+        text_ids = tok.encode(text.strip() + "\n", add_special_tokens=False)
+        n_lm = int(cached_prompt["lm"]["last_hidden_state"].size(1))
+        n_tts = int(cached_prompt["tts_lm"]["last_hidden_state"].size(1))
+        cols = {"input_ids": [[tok.pad_id] * n_lm], "tts_lm_input_ids": [[tok.pad_id] * n_tts], "tts_text_ids": [list(text_ids)]}
+        if return_attention_mask:
+            cols["attention_mask"] = [[1] * n_lm]
+            cols["tts_lm_attention_mask"] = [[1] * n_tts]
+        out = BatchEncoding()
+        for k, v in cols.items():
+            out[k] = torch.tensor(v, dtype=torch.long) if return_tensors is not None else v
+        out["speech_input_mask"] = torch.zeros(1, n_tts, dtype=torch.bool) if return_tensors is not None else [[False] * n_tts]
+        out["speech_tensors"] = out["speech_masks"] = None
+        return out
+
+    save_audio = VibeVoiceProcessor.save_audio
+    batch_decode = VibeVoiceProcessor.batch_decode
+    decode = VibeVoiceProcessor.decode

@@ -6,13 +6,17 @@ What differs from the multi-speaker loop (`modeling.py`), and how it maps onto t
     LM" with the final norm.  Both live in the engine's one layer array (lower first); `vv_lm_decode_range` runs one stack at a time.
     Each stack has its own KV sequences because their lengths differ (the upper stack also sees the speech positions):
         row 0 = TTS-LM positive stream, row 1 = lower text stack, row 2 = TTS-LM negative stream (max_batch = 2, row 3 unused);
-  * every TTS-LM input gets a type embedding added (1 = text, 0 = speech; `:290-291`);
+  * every TTS-LM input gets a type embedding added (1 = text, 0 = speech; `:290-291`): `vv_tts_type_embed`;
   * no token selection: windows of 5 text tokens alternate with 6 speech frames (`:40-42, :568-614`); a binary classifier on the TTS-LM
-    hidden state ends the utterance (`:691-696`);
+    hidden state ends the utterance (`:691-696`): `vv_eos_prob`, whose result is the one host sync per speech frame;
   * no semantic tokenizer: the frame is sampler -> acoustic decoder -> acoustic connector (`:617-645`).  The engine is given zero
     semantic weights, for which its connector stage returns exactly `acoustic_connector(latent)` (RMSNorm(0) = 0), and the semantic
     encoder stage is simply never launched.
 Batch size 1, like the reference (`:511`).
+
+The native `Engine` always runs the type embeddings and the EOS classifier on its sm_90a kernels (`vv_tts_type_embed`, `vv_eos_prob`),
+and a checkpoint without their weights is refused.  An engine object that does not implement them (no `has_tts_heads`: the CPU
+stand-in the host-logic tests drive this loop with, whose contract predates these kernels) gets the same two ops in fp32 PyTorch here.
 
 STATUS: host logic held to fixtures from the reference's own streaming generate() on the CPU through the engine stand-in
 (`tests/test_host_logic.py::test_streaming_product_host_logic_against_reference_fixture`); CUDA path vs the pinned oracle on the GPU
@@ -36,11 +40,13 @@ TTS_TEXT_WINDOW_SIZE = 5      # :41
 TTS_SPEECH_WINDOW_SIZE = 6    # :42
 ROW_POS, ROW_TEXT, ROW_NEG = 0, 1, 2
 LM, TTS = "model.language_model", "model.tts_language_model"
+HEAD_NAMES = ("model.tts_input_types.weight", "tts_eos_classifier.fc1.weight", "tts_eos_classifier.fc1.bias", "tts_eos_classifier.fc2.weight",
+              "tts_eos_classifier.fc2.bias")
 
 
 def remap_streaming_state_dict(items: Iterable[Tuple[str, torch.Tensor]], config: VibeVoiceConfig, tts_layers: int):
-    """Streaming checkpoint keys -> the engine's (multi-speaker) names; yields (name, tensor).  Also returns, through the generator's
-    `extras` dict, the streaming-only modules that stay on the host side of the boundary (type embeddings, EOS classifier)."""
+    """Streaming checkpoint keys -> the engine's (multi-speaker) names; yields (name, tensor).  The streaming-only modules (type
+    embeddings, EOS classifier) keep their names: the engine loads them as optional tensors."""
     low = config.decoder_config.num_hidden_layers - tts_layers
     for k, v in items:
         if k.startswith(TTS + ".layers."):
@@ -64,8 +70,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
         self._device_index, self._max_steps = device, max_diffusion_steps
         self.engine: Optional[Engine] = None
         self.ddpm_inference_steps = config.diffusion_head_config.ddpm_num_inference_steps
-        self.types: Optional[torch.Tensor] = None              # tts_input_types.weight [2, H]
-        self.eos: Dict[str, torch.Tensor] = {}                 # tts_eos_classifier.{fc1,fc2}.{weight,bias}
+        self._host_heads: Optional[Dict[str, torch.Tensor]] = None   # only for engines without vv_tts_type_embed / vv_eos_prob
 
     def set_ddpm_inference_steps(self, num_steps=None):
         self.ddpm_inference_steps = num_steps or self.config.diffusion_head_config.ddpm_num_inference_steps
@@ -121,15 +126,14 @@ class VibeVoiceStreamingForConditionalGenerationInference:
         scale = bias = None
         seen_sem = False
         shapes: Dict[str, Tuple[torch.Size, torch.dtype]] = {}
+        heads: Dict[str, torch.Tensor] = {}
         for name, t in remap_streaming_state_dict(items, self.config, self.tts_layers):
             if name == "model.speech_scaling_factor":
                 scale = float(t)
             elif name == "model.speech_bias_factor":
                 bias = float(t)
-            elif name == "model.tts_input_types.weight":
-                self.types = t.to(device=eng.device, dtype=torch.float32)
-            elif name.startswith("tts_eos_classifier."):
-                self.eos[name[len("tts_eos_classifier."):]] = t.to(device=eng.device, dtype=torch.float32)
+            elif name in HEAD_NAMES:
+                heads[name] = t
             else:
                 seen_sem |= name.startswith("model.semantic")
                 eng.load_tensor(name, t)
@@ -138,9 +142,14 @@ class VibeVoiceStreamingForConditionalGenerationInference:
             for name, shape, _ in param_specs(self.config):
                 if name.startswith("model.semantic"):
                     eng.load_tensor(name, torch.zeros(*shape, dtype=torch.bfloat16))
+        native = hasattr(type(eng), "has_tts_heads")                # the engine implements the head kernels
+        if native:
+            for name, t in heads.items():
+                eng.load_tensor(name, t)
         eng.finalize(scale, bias)
-        if self.types is None or len(self.eos) != 4:
+        if not (eng.has_tts_heads if native else len(heads) == len(HEAD_NAMES)):
             raise N.VVError("streaming checkpoint lacks model.tts_input_types / tts_eos_classifier")
+        self._host_heads = None if native else {k: v.to(device=eng.device, dtype=torch.float32) for k, v in heads.items()}
         return self
 
     # ---- building blocks of the loop ----------------------------------------------------------------------------------
@@ -153,8 +162,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
             eng.set_row_mode([0, 1, 0, 0])
             eng.lm_decode_range(0, self.low, False)
             eng.kv_commit([0, 1, 0, 0])
-            with torch.cuda.stream(eng.stream):
-                eng.embeds[up_row].copy_(eng.hidden[ROW_TEXT] + self.types[1])
+            self._type_embed(eng.hidden[ROW_TEXT], 1, [up_row])
             eng.set_row_mode([1 if r == up_row else 0 for r in range(4)])
             eng.lm_decode_range(self.low, self.low + self.tts_layers, True)
             eng.kv_commit([1 if r == up_row else 0 for r in range(4)])
@@ -162,21 +170,31 @@ class VibeVoiceStreamingForConditionalGenerationInference:
     def _speech_step(self, embed: torch.Tensor):
         """One TTS-LM step on both streams with the acoustic embedding (+ type 0) (:657-689)."""
         eng = self.engine
-        with torch.cuda.stream(eng.stream):
-            x = embed + self.types[0]
-            eng.embeds[ROW_POS].copy_(x)
-            eng.embeds[ROW_NEG].copy_(x)
+        self._type_embed(embed, 0, [ROW_POS, ROW_NEG])
         eng.set_row_mode([1, 0, 1, 0])
         eng.lm_decode_range(self.low, self.low + self.tts_layers, True)
         eng.kv_commit([1, 0, 1, 0])
 
-    def _eos_prob(self) -> float:
-        """`sigmoid(tts_eos_classifier(h))` (:691; BinaryClassifier, modeling_vibevoice_streaming.py:42-53) -- two tiny products."""
+    def _type_embed(self, src: torch.Tensor, type_id: int, rows: List[int]):
+        """`embeds[r] = src + tts_input_types[type_id]` for r in rows (:290-291); src may be one of those rows."""
         eng = self.engine
+        if self._host_heads is None:
+            eng.tts_type_embed(src, type_id, rows, eng.embeds)
+            return
         with torch.cuda.stream(eng.stream):
-            h = eng.hidden[ROW_POS]
-            x = torch.relu(self.eos["fc1.weight"] @ h + self.eos["fc1.bias"])
-            p = torch.sigmoid(self.eos["fc2.weight"] @ x + self.eos["fc2.bias"])
+            x = src + self._host_heads["model.tts_input_types.weight"][type_id]
+            for r in rows:
+                eng.embeds[r].copy_(x)
+
+    def _eos_prob(self) -> float:
+        """`sigmoid(tts_eos_classifier(h))` (:691; BinaryClassifier, modeling_vibevoice_streaming.py:42-53), one host sync."""
+        eng = self.engine
+        if self._host_heads is None:
+            return eng.eos_prob(eng.hidden[ROW_POS])
+        w = self._host_heads
+        with torch.cuda.stream(eng.stream):
+            x = torch.relu(w["tts_eos_classifier.fc1.weight"] @ eng.hidden[ROW_POS] + w["tts_eos_classifier.fc1.bias"])
+            p = torch.sigmoid(w["tts_eos_classifier.fc2.weight"] @ x + w["tts_eos_classifier.fc2.bias"])
         eng.sync()
         return float(p[0])
 
@@ -301,9 +319,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
                 seq.append(1)                                                                      # :646
                 if len(seq) > max_length:                                                          # :648-649
                     break
-                with torch.cuda.stream(eng.stream):
-                    emb = eng.embeds[ROW_POS].clone()
-                self._speech_step(emb)
+                self._speech_step(eng.embeds[ROW_POS])
                 if self._eos_prob() > 0.5:                                                         # :691-696
                     finished = True
                     if audio_streamer is not None:
