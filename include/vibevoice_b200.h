@@ -205,15 +205,16 @@ int vv_eos_prob(vv_ctx* ctx, const float* hidden, float* prob_out, float* logit_
 /* the inverse of vv_kv_write: K / V [n][kv_heads][head_dim] bf16 of positions [pos0, pos0 + n) of (seq, layer); either output may be NULL */
 int vv_debug_kv_read(vv_ctx* ctx, int seq, int layer, int64_t pos0, int64_t n, void* k_out, void* v_out, void* stream);
 int64_t vv_launch_count(vv_ctx* ctx);     /* kernels launched by this ctx so far */
-int vv_debug_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, float* y, int M, int N, int K,
-                  int prologue, const float* pro_w, float eps, int epilogue, void* stream);
-/* the same dispatch (GEMV, tensor-core GEMMs, wgmma) with every feature the codec passes use: y[m][n] = epi(W pro(x_m) + bias[n]).
- * Row m = (b, t) = (m / map_T, m % map_T) of x starts at x + b * map_bs + t * ldx floats (map_T = 0: dense rows ldx apart); rows may
- * overlap, which is how a convolution reads its window.  prologue: 0 none, 1 RMSNorm(pro_w, eps), 3 SiLU.  epilogue: 0 none, 2 + res,
- * 3 res + epi_a[m][n] (rows epi_lda apart) *, 4 res + epi_a[n] *, 6 GELU, 7 SiLU; res rows ldres apart; res == y with ldres == ldy runs
- * in place, and on grids smaller than the GPU the tensor-core GEMMs then split K and add into y with fp32 atomics.  info[2] = {kernel,
- * split-K factor}: kernel 0 GEMV, 1..7 gemm_mma_ring_kernel <1,GELU> <1,NONE> <0,GAMMA_RESID> <0,NONE> <0,GELU> <0,RESID> <-1,-1>,
- * 8 gemm_mma_kernel, 9 split_bf16_kernel + gemm_wgmma_kernel.  Needs vv_finalize_weights (VV_ERR_STATE).  Synchronises. */
+/* linear(), the GEMM dispatch of the kernel-per-stage path (GEMV, tensor-core GEMMs, wgmma), with every feature the codec passes use:
+ * y[m][n] = epi(W pro(x_m) + bias[n]).  Row m = (b, t) = (m / map_T, m % map_T) of x starts at x + b * map_bs + t * ldx floats
+ * (map_T = 0: dense rows ldx apart); rows may overlap, which is how a convolution reads its window.  prologue: 0 none, 1 RMSNorm(pro_w,
+ * eps).  epilogue: 0 none, 2 + res, 4 res + epi_a[n] * (W pro(x_m) + bias[n]), 6 GELU, 7 SiLU; res rows ldres apart; res == y with
+ * ldres == ldy runs in place, and on grids smaller than the GPU the tensor-core GEMMs then split K and add into y with fp32 atomics.
+ * epi_lda is ignored (no epilogue reads a per-row operand; the argument keeps existing callers' argument lists valid).  info[2] =
+ * {kernel, split-K factor}: kernel 0 GEMV, 1..7 gemm_mma_ring_kernel <1,GELU> <1,NONE> <0,GAMMA_RESID> <0,NONE> <0,GELU> <0,RESID>
+ * <-1,-1>, 9 split_bf16_kernel + gemm_wgmma_kernel (8 is retired).  Refused with VV_ERR_INVALID, nothing launched: any other prologue or
+ * epilogue, and RMSNorm at M >= 9 with K > 512 or with a K split (the tensor-core GEMM folds the norm in only without them).  Needs
+ * vv_finalize_weights (VV_ERR_STATE).  Synchronises. */
 int vv_debug_gemv2(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, int64_t ldx, int map_T, int64_t map_bs, float* y,
                    int64_t ldy, const float* res, int64_t ldres, int M, int N, int K, int prologue, const float* pro_w, float eps,
                    int epilogue, const float* epi_a, int64_t epi_lda, int32_t* info, void* stream);
@@ -269,15 +270,12 @@ int vv_debug_voice_taps(vv_ctx* ctx, const float* wavs, int n, int64_t T, const 
                         void* workspace, int64_t workspace_bytes, float* taps, int64_t taps_floats, int32_t* meta, void* stream);
 
 int vv_debug_barrier_bench(vv_ctx* ctx, int iters, int ctas_per_sm, float* ms_out);
-/* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh): y = [y +] alpha * (W pro(x) + bias).
- * prologue: 0 none, 1 RMSNorm(pro_w, eps), 3 SwiGLU pairs (x is [M][2K]), 4 GELU, 6 SiLU; alpha_kind: 0 one, 2 gamma[n]. Synchronises. */
-int vv_debug_stream_gemv(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, float* y, int M, int N, int K, int prologue,
-                         const float* pro_w, float eps, int alpha_kind, const float* alpha, int accumulate, void* stream);
-/* the same linear with every stage feature exposed: y[m][n] = (store ? 0 : y[m][n]) + alpha * (W pro(x[m]) + bias[n]), rows of x / y
- * ldx / ldy floats apart (SwiGLU: x rows hold 2K interleaved gate / up sums).  prologue 2 = AdaLN: RMSNorm(pro_w or 1, eps) * (1 + scale) +
- * shift with scale / shift rows pro_ld floats apart; alpha_kind 1 = gate alpha[m][n] (row stride lda), 2 = gamma alpha[n].  store needs
- * K <= 64.  operand_cap > 0 caps the activation-operand bytes of the stage, so that smaller shapes run through the K split as well.
- * Synchronises; returns the number of stages the linear ran as (> 1: split along K). */
+/* one linear through the persistent weight-stream kernel (wgmma + TMA, csrc/vv_stream.cuh) with every stage feature exposed:
+ * y[m][n] = (store ? 0 : y[m][n]) + alpha * (W pro(x[m]) + bias[n]), rows of x / y ldx / ldy floats apart.  prologue: 0 none,
+ * 1 RMSNorm(pro_w, eps), 2 AdaLN: RMSNorm(pro_w or 1, eps) * (1 + scale) + shift with scale / shift rows pro_ld floats apart, 3 SwiGLU
+ * pairs (x rows hold 2K interleaved gate / up sums), 4 GELU, 6 SiLU; alpha_kind: 0 one, 1 gate alpha[m][n] (row stride lda), 2 gamma
+ * alpha[n].  store needs K <= 64.  operand_cap > 0 caps the activation-operand bytes of the stage, so that smaller shapes run through the
+ * K split as well.  Synchronises; returns the number of stages the linear ran as (> 1: split along K). */
 int vv_debug_stream_gemv2(vv_ctx* ctx, const void* w_bf16, const float* bias, const float* x, int64_t ldx, float* y, int64_t ldy, int M, int N,
                           int K, int prologue, const float* pro_w, float eps, const float* pro_shift, const float* pro_scale, int64_t pro_ld,
                           int alpha_kind, const float* alpha, int64_t lda, int store, int64_t operand_cap, void* stream);

@@ -428,10 +428,10 @@ def test_codec_taps_errors():
 
 
 # ---- GPU: vv_debug_gemv2, the GEMM dispatch of the kernel-per-stage path -----------------------------------------------------------------
-PRO_NONE, PRO_RMSNORM, PRO_SILU = 0, 1, 3
-EPI_NONE, EPI_RESID, EPI_GATED_RESID, EPI_GAMMA_RESID, EPI_GELU, EPI_SILU = 0, 2, 3, 4, 6, 7
-KERNELS = ["gemv", "ring<1,GELU>", "ring<1,NONE>", "ring<0,GAMMA_RESID>", "ring<0,NONE>", "ring<0,GELU>", "ring<0,RESID>", "ring<-1,-1>",
-           "gemm_mma", "wgmma"]
+PRO_NONE, PRO_RMSNORM = 0, 1
+EPI_NONE, EPI_RESID, EPI_GAMMA_RESID, EPI_GELU, EPI_SILU = 0, 2, 4, 6, 7
+KERNELS = {0: "gemv", 1: "ring<1,GELU>", 2: "ring<1,NONE>", 3: "ring<0,GAMMA_RESID>", 4: "ring<0,NONE>", 5: "ring<0,GELU>", 6: "ring<0,RESID>",
+           7: "ring<-1,-1>", 9: "wgmma"}
 SENTINEL = 12345.0
 
 
@@ -457,7 +457,6 @@ GEMV2_CASES = {
     "ring_rms_gelu_m9_k512": (9, 200, 512, PRO_RMSNORM, EPI_GELU, None, "ring<1,GELU>"),
     "ring_rms_gelu_m33_k504": (33, 130, 504, PRO_RMSNORM, EPI_GELU, None, "ring<1,GELU>"),
     "ring_rms_none_m32": (32, 63, 264, PRO_RMSNORM, EPI_NONE, None, "ring<1,NONE>"),
-    "mma_rms_gelu_k520": (33, 130, 520, PRO_RMSNORM, EPI_GELU, None, "gemm_mma"),
     "ring_gamma_inplace_split1": (32, 96, 448, PRO_NONE, EPI_GAMMA_RESID, "inplace", "ring<0,GAMMA_RESID>"),
     "ring_gamma_inplace_split2": (32, 6400, 512, PRO_NONE, EPI_GAMMA_RESID, "inplace", "ring<0,GAMMA_RESID>"),
     "ring_gamma_inplace_split16": (33, 256, 2056, PRO_NONE, EPI_GAMMA_RESID, "inplace", "ring<0,GAMMA_RESID>"),
@@ -469,9 +468,6 @@ GEMV2_CASES = {
     "ring_resid_inplace_split8": (32, 128, 1024, PRO_NONE, EPI_RESID, "inplace", "ring<0,RESID>"),
     "ring_generic_silu": (20, 100, 96, PRO_NONE, EPI_SILU, None, "ring<-1,-1>"),
     "ring_generic_rms_gamma": (24, 100, 256, PRO_RMSNORM, EPI_GAMMA_RESID, "separate", "ring<-1,-1>"),
-    "ring_generic_gated": (24, 100, 128, PRO_NONE, EPI_GATED_RESID, "separate", "ring<-1,-1>"),
-    "mma_silu": (12, 100, 128, PRO_SILU, EPI_NONE, None, "gemm_mma"),
-    "mma_rms_gamma_inplace_split8": (32, 128, 1024, PRO_RMSNORM, EPI_GAMMA_RESID, "inplace", "gemm_mma"),
     "wgmma_gamma_inplace": (200, 4000, 520, PRO_NONE, EPI_GAMMA_RESID, "inplace", "wgmma"),
     "wgmma_none_m65": (65, 12300, 136, PRO_NONE, EPI_NONE, None, "wgmma"),
     "convtr_window": (None, 160, convtr_map(2, 40, 64), PRO_NONE, EPI_NONE, None, "ring<0,NONE>"),
@@ -516,32 +512,27 @@ def test_gemv2_vs_float64(tiny2, case):
     W = (torch.randn(N, K, generator=g) * 0.05).to(torch.bfloat16)
     bias, nw = torch.randn(N, generator=g) * 0.1, torch.rand(K, generator=g) + 0.5
     gam = torch.rand(N, generator=g) + 0.5
-    ldy, lda = N + 5, N + 3
-    gate = torch.full((M, lda), float("nan"))
-    gate[:, :N] = torch.rand(M, N, generator=g) + 0.5
-    res = torch.full((M, lda), float("nan"))
+    ldy, ldr = N + 5, N + 3
+    res = torch.full((M, ldr), float("nan"))
     res[:, :N] = torch.randn(M, N, generator=g)
     y = torch.full((M + 3, ldy), SENTINEL)
     y[:M, :N] = res[:, :N] if resid == "inplace" else float("nan")
-    d = {k: v.cuda() for k, v in dict(W=W, bias=bias, nw=nw, gam=gam, gate=gate, res=res, x=x, y=y).items()}
+    d = {k: v.cuda() for k, v in dict(W=W, bias=bias, nw=nw, gam=gam, res=res, x=x, y=y).items()}
     P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-    rp, ldres = (d["y"], ldy) if resid == "inplace" else ((d["res"], lda) if resid else (None, 0))
-    ea = d["gam"] if epi == EPI_GAMMA_RESID else (d["gate"] if epi == EPI_GATED_RESID else None)
+    rp, ldres = (d["y"], ldy) if resid == "inplace" else ((d["res"], ldr) if resid else (None, 0))
+    ea = d["gam"] if epi == EPI_GAMMA_RESID else None
     info = np.zeros(2, dtype=np.int32)
     torch.cuda.synchronize()
     NV.check(eng.lib.vv_debug_gemv2(eng.h, P(d["W"]), P(d["bias"]), P(d["x"]), ldx, T, bs, P(d["y"]), ldy, P(rp), ldres, M, N, K, pro,
-                                    P(d["nw"]), 1e-5, epi, P(ea), lda, NV.iptr(info), eng.s), "vv_debug_gemv2")
+                                    P(d["nw"]), 1e-5, epi, P(ea), 0, NV.iptr(info), eng.s), "vv_debug_gemv2")
     got = d["y"].cpu()
     # float64 reference
     xr = x.double()[offs[:, None] + torch.arange(K)[None, :]]
     if pro == PRO_RMSNORM:
         xr = _rms(xr, nw.double(), 1e-5)
-    elif pro == PRO_SILU:
-        xr = F.silu(xr)
     lin = xr @ W.double().T + bias.double()
     r0 = res[:, :N].double()
-    ref = {EPI_NONE: lin, EPI_GELU: F.gelu(lin), EPI_SILU: F.silu(lin), EPI_RESID: r0 + lin, EPI_GAMMA_RESID: r0 + gam.double() * lin,
-           EPI_GATED_RESID: r0 + gate[:, :N].double() * lin}[epi]
+    ref = {EPI_NONE: lin, EPI_GELU: F.gelu(lin), EPI_SILU: F.silu(lin), EPI_RESID: r0 + lin, EPI_GAMMA_RESID: r0 + gam.double() * lin}[epi]
     out = got[:M, :N].double()
     assert not torch.isnan(out).any(), "NaN in the output (input padding read, or an element not written)"
     assert torch.equal(got[:M, N:], torch.full_like(got[:M, N:], SENTINEL)), "write past N into the row padding of y"
@@ -549,8 +540,47 @@ def test_gemv2_vs_float64(tiny2, case):
     e = float((out - ref).norm() / ((ref - r0).norm() if resid else ref.norm()))
     G = torch.cuda.get_device_properties(0).multi_processor_count
     split = expected_split(M, N, K, resid == "inplace", kernel, G)
-    report("codec_gemv2", case=case, M=M, N=N, K=K, kernel=KERNELS[info[0]], split_k=int(info[1]), rel_l2=e)
-    assert (KERNELS[info[0]], int(info[1])) == (kernel, split), (case, KERNELS[info[0]], int(info[1]), kernel, split)
+    report("codec_gemv2", case=case, M=M, N=N, K=K, kernel=KERNELS[int(info[0])], split_k=int(info[1]), rel_l2=e)
+    assert (KERNELS[int(info[0])], int(info[1])) == (kernel, split), (case, int(info[0]), int(info[1]), kernel, split)
     if case.endswith("split2") or case.endswith("split8") or case.endswith("split16"):
         assert split == int(case.rsplit("split", 1)[1]), (case, split, G)
     assert e < 2e-5, (case, e)
+
+
+# name: (M, N, K, prologue, epilogue, residual, what vv_last_error names).  linear() has no kernel for these: the AdaLN (2) and SiLU (3)
+# prologues, the gated-residual (3) and SwiGLU (5) epilogues, and RMSNorm at M >= 9 that the ring cannot fold in (K > 512, or K split by an
+# in-place residual).
+GEMV2_REFUSED = {
+    "mma_rms_gelu_k520": (33, 130, 520, PRO_RMSNORM, EPI_GELU, None, "RMSNorm at M=33"),
+    "mma_silu": (12, 100, 128, 3, EPI_NONE, None, "prologue 3"),
+    "mma_rms_gamma_inplace_split8": (32, 128, 1024, PRO_RMSNORM, EPI_GAMMA_RESID, "inplace", "RMSNorm at M=32"),
+    "ring_generic_gated": (24, 100, 128, PRO_NONE, 3, "separate", "epilogue 3"),
+    "gemv_adaln": (2, 64, 256, 2, EPI_NONE, None, "prologue 2"),
+    "gemv_swiglu": (2, 64, 256, PRO_RMSNORM, 5, None, "epilogue 5"),
+    "rms_none_k520": (16, 512, 520, PRO_RMSNORM, EPI_NONE, None, "RMSNorm at M=16"),
+    "rms_gamma_inplace_k512_split4": (32, 128, 512, PRO_RMSNORM, EPI_GAMMA_RESID, "inplace", "split 4"),
+}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", list(GEMV2_REFUSED))
+def test_gemv2_refuses(tiny2, case):
+    """A case linear() has no kernel for returns VV_ERR_INVALID, says which case in vv_last_error, launches nothing and leaves y alone."""
+    eng = tiny2[0].engine
+    M, N, K, pro, epi, resid, msg = GEMV2_REFUSED[case]
+    d = dict(W=torch.zeros(N, K, dtype=torch.bfloat16), x=torch.ones(M, K), nw=torch.ones(K), gam=torch.ones(N), res=torch.zeros(M, N),
+             y=torch.full((M, N), SENTINEL))
+    d = {k: v.cuda() for k, v in d.items()}
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+    rp = d["y"] if resid == "inplace" else (d["res"] if resid else None)
+    info = np.full(2, -1, dtype=np.int32)
+    torch.cuda.synchronize()
+    before = eng.launch_count()
+    rc = eng.lib.vv_debug_gemv2(eng.h, P(d["W"]), None, P(d["x"]), K, 0, 0, P(d["y"]), N, P(rp), N if rp is not None else 0, M, N, K, pro,
+                                P(d["nw"]), 1e-5, epi, P(d["gam"]), 0, NV.iptr(info), eng.s)
+    err = eng.lib.vv_last_error().decode()
+    assert rc == -1 and err.startswith("linear: ") and msg in err, (case, rc, err)
+    assert eng.launch_count() == before
+    torch.cuda.synchronize()
+    assert torch.equal(d["y"].cpu(), torch.full((M, N), SENTINEL)), case
+    assert list(info) == [-1, -1], info

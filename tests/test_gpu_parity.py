@@ -63,7 +63,7 @@ def small1():
 @pytest.mark.parametrize("M,N,K", [(1, 64, 256), (2, 1536, 1536), (2, 2048, 1536), (2, 4608, 1536), (2, 1536, 8960),
                                    (4, 320, 448), (8, 1024, 2048), (3, 100, 264), (16, 512, 1024), (2, 64, 18944),
                                    (40, 2048, 512), (200, 1024, 256), (70, 96, 40)])
-def test_gemv_matches_torch(tiny2, M, N, K):
+def test_gemv2_matches_torch(tiny2, M, N, K):
     """The weight-streaming GEMV / tiled GEMM against a plain PyTorch fp32 reference of the same op."""
     import ctypes as C
     eng = tiny2[0].engine
@@ -73,29 +73,30 @@ def test_gemv_matches_torch(tiny2, M, N, K):
     bias = torch.randn(N, generator=g) * 0.1
     nw = torch.rand(K, generator=g) + 0.5
     Wd, xd, bd, nwd = W.cuda(), x.cuda(), bias.cuda(), nw.cuda()
-    P = lambda t: C.c_void_p(t.data_ptr())
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+    info = np.zeros(2, dtype=np.int32)
     cases = [(NV.PRO_NONE, NV.EPI_NONE), (NV.PRO_NONE, NV.EPI_GELU), (NV.PRO_NONE, NV.EPI_SILU), (NV.PRO_RMSNORM, NV.EPI_GELU),
-             (NV.PRO_SILU, NV.EPI_NONE), (NV.PRO_RMSNORM, NV.EPI_SWIGLU), (NV.PRO_NONE, NV.EPI_RESID)]
+             (NV.PRO_NONE, NV.EPI_RESID)]
     for pro, epi in cases:
-        if epi == NV.EPI_SWIGLU and N % 2:
-            continue
-        y = torch.full((M, N // 2 if epi == NV.EPI_SWIGLU else N), 0.25, device="cuda")
+        y = torch.full((M, N), 0.25, device="cuda")
         y0 = y.clone()
-        with torch.cuda.stream(eng.stream):
-            NV.check(eng.lib.vv_debug_gemv(eng.h, P(Wd), P(bd), P(xd), P(y), M, N, K, pro, P(nwd), 1e-5, epi, eng.s))
-        eng.sync()
+        res = y if epi == NV.EPI_RESID else None
+        torch.cuda.synchronize()
+        rc = eng.lib.vv_debug_gemv2(eng.h, P(Wd), P(bd), P(xd), K, 0, 0, P(y), N, P(res), N if res is not None else 0, M, N, K, pro, P(nwd),
+                                    1e-5, epi, None, 0, NV.iptr(info), eng.s)
+        if pro == NV.PRO_RMSNORM and M >= 9 and K > 512:
+            # above the GEMV's 8 rows RMSNorm is folded into the tensor-core GEMM, which stages the norm weight for K <= 512 only
+            assert rc == -1 and torch.equal(y, y0), (M, N, K, rc)
+            continue
+        NV.check(rc, "vv_debug_gemv2")
         xt = x.clone()
         if pro == NV.PRO_RMSNORM:
             xt = xt * torch.rsqrt(xt.pow(2).mean(-1, keepdim=True) + 1e-5) * nw
-        elif pro == NV.PRO_SILU:
-            xt = torch.nn.functional.silu(xt)
         ref = xt @ W.float().T + bias
         if epi == NV.EPI_GELU:
             ref = torch.nn.functional.gelu(ref)
         elif epi == NV.EPI_SILU:
             ref = torch.nn.functional.silu(ref)
-        elif epi == NV.EPI_SWIGLU:
-            ref = torch.nn.functional.silu(ref[:, 0::2]) * ref[:, 1::2]
         elif epi == NV.EPI_RESID:
             ref = ref + y0.cpu()
         e = rel_l2(y, ref)
@@ -678,7 +679,7 @@ def test_voice_prompt_and_torch_prefill_vs_oracle():
     model.engine.close()
 
 
-def test_wgmma_gemm_forced_everywhere():
+def test_gemv2_wgmma_forced_everywhere():
     """gemm_wgmma_kernel (warpgroup wgmma.mma_async, register accumulators) is selected automatically only for wide GEMMs; force it for
     EVERY M > 8 GEMM (VV_WGMMA=2) and re-check the GEMM-vs-torch cases and a closed codec loop through the tensor-core path."""
     import ctypes as C
@@ -692,7 +693,8 @@ def test_wgmma_gemm_forced_everywhere():
         else:
             os.environ["VV_WGMMA"] = old
     eng = m.engine
-    P = lambda t: C.c_void_p(t.data_ptr())
+    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+    info = np.zeros(2, dtype=np.int32)
     for (M, N, K) in [(40, 2048, 512), (200, 1024, 256), (70, 96, 40), (60, 21504, 1536), (130, 200, 72)]:
         g = torch.Generator().manual_seed(M + N + K)
         W = (torch.randn(N, K, generator=g) * 0.05).to(torch.bfloat16)
@@ -701,10 +703,11 @@ def test_wgmma_gemm_forced_everywhere():
         torch.cuda.synchronize()
         for epi in (NV.EPI_NONE, NV.EPI_GELU, NV.EPI_RESID):
             y = torch.full((M, N), 0.25, device="cuda")
+            res = y if epi == NV.EPI_RESID else None
             torch.cuda.synchronize()
-            with torch.cuda.stream(eng.stream):
-                NV.check(eng.lib.vv_debug_gemv(eng.h, P(Wd), P(bd), P(xd), P(y), M, N, K, NV.PRO_NONE, None, 1e-5, epi, eng.s))
-            eng.sync()
+            NV.check(eng.lib.vv_debug_gemv2(eng.h, P(Wd), P(bd), P(xd), K, 0, 0, P(y), N, P(res), N if res is not None else 0, M, N, K,
+                                            NV.PRO_NONE, None, 1e-5, epi, None, 0, NV.iptr(info), eng.s), "vv_debug_gemv2")
+            assert int(info[0]) == 9, (M, N, K, epi, int(info[0]))     # 9: split_bf16_kernel + gemm_wgmma_kernel
             ref = x @ W.float().T + bias
             ref = torch.nn.functional.gelu(ref) if epi == NV.EPI_GELU else (ref + 0.25 if epi == NV.EPI_RESID else ref)
             e = rel_l2(y, ref)

@@ -21,7 +21,7 @@ SHAPES = [(2, 1536, 1536), (2, 2048, 1536), (2, 17920, 1536), (2, 1536, 8960), (
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
-def test_stream_gemv_matches_torch(tiny2, M, N, K):
+def test_stream_gemv2_matches_torch(tiny2, M, N, K):
     eng = tiny2[0].engine
     g = torch.Generator().manual_seed(M * 1000003 + N * 101 + K)
     W = (torch.randn(N, K, generator=g) * 0.05).to(torch.bfloat16)
@@ -33,12 +33,13 @@ def test_stream_gemv_matches_torch(tiny2, M, N, K):
     cases = [(SP_NONE, SA_ONE, False, True), (SP_RMSNORM, SA_ONE, False, False), (SP_SWIGLU, SA_ONE, True, False),
              (SP_GELU, SA_GAMMA, True, True), (SP_SILU, SA_ONE, False, True)]
     for pro, ak, accumulate, with_bias in cases:
-        x = torch.randn(M, 2 * K if pro == SP_SWIGLU else K, generator=g)
+        Kx = 2 * K if pro == SP_SWIGLU else K
+        x = torch.randn(M, Kx, generator=g)
         xd = x.cuda()
-        y = torch.full((M, N), 0.25, device="cuda")
+        y = torch.full((M, N), 0.25 if accumulate else 0.0, device="cuda")      # not accumulating: into a zeroed y
         torch.cuda.synchronize()
-        NV.check(eng.lib.vv_debug_stream_gemv(eng.h, P(Wd), P(bd) if with_bias else None, P(xd), P(y), M, N, K, pro, P(nwd), 1e-5, ak,
-                                              P(gamd) if ak == SA_GAMMA else None, int(accumulate), eng.s), "vv_debug_stream_gemv")
+        NV.check(eng.lib.vv_debug_stream_gemv2(eng.h, P(Wd), P(bd) if with_bias else None, P(xd), Kx, P(y), N, M, N, K, pro, P(nwd), 1e-5,
+                                               None, None, 0, ak, P(gamd) if ak == SA_GAMMA else None, N, 0, 0, eng.s), "vv_debug_stream_gemv2")
         xt = x
         if pro == SP_RMSNORM:
             xt = x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + 1e-5) * nw

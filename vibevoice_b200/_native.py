@@ -14,8 +14,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libvibevoice_b200.so")
 
 VV_DT_BF16, VV_DT_F32, VV_DT_F16 = 0, 1, 2
-PRO_NONE, PRO_RMSNORM, PRO_ADALN, PRO_SILU = 0, 1, 2, 3
-EPI_NONE, EPI_RESID, EPI_GATED_RESID, EPI_GAMMA_RESID, EPI_SWIGLU, EPI_GELU, EPI_SILU = 0, 2, 3, 4, 5, 6, 7
+PRO_NONE, PRO_RMSNORM = 0, 1
+EPI_NONE, EPI_RESID, EPI_GAMMA_RESID, EPI_GELU, EPI_SILU = 0, 2, 4, 6, 7
 
 
 class VVError(RuntimeError):
@@ -84,13 +84,11 @@ SYMBOLS = {
     "vv_debug_kv_read": (_I, [_P, _I, _I, _L, _L, _P, _P, _P]),
     "vv_launch_count": (_L, [_P]),
     "vv_debug_barrier_bench": (_I, [_P, _I, _I, C.POINTER(C.c_float)]),
-    "vv_debug_gemv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _F, _I, _P]),
     "vv_debug_gemv2": (_I, [_P, _P, _P, _P, _L, _I, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _F, _I, _P, _L, _P, _P]),
     "vv_debug_codec_taps": (_I, [_P, _I, _P, _P, _P, _P, _L, _P, _P]),
     "vv_debug_sampler_taps": (_I, [_P, _P, _P, _F, _P, _P, _L, _P, _P]),
     "vv_debug_prefill_taps": (_I, [_P, _I, _L, _L, _I, _P, _P, _P, _L, _P, _L, _P, _P]),
     "vv_debug_voice_taps": (_I, [_P, _P, _I, _L, _P, _P, _P, _P, _L, _P, _L, _P, _P]),
-    "vv_debug_stream_gemv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _F, _I, _P, _I, _P]),
     "vv_debug_stream_gemv2": (_I, [_P, _P, _P, _P, _L, _P, _L, _I, _I, _I, _I, _P, _F, _P, _P, _L, _I, _P, _L, _I, _L, _P]),
     "vv_stream_diag": (_I, [_P, _P]),
     "vv_stream_trace_read": (_I, [_P, _P, _P, _I, C.c_char_p]),

@@ -7,10 +7,10 @@
 // prologue and epilogue so no activation round-trips through HBM more than once.
 //
 // Reference anchors (under vibevoice/modular of the reference project unless noted):
-//   gemv prologues RMSNORM/ADALN      modular_vibevoice_diffusion_head.py:31-45, 158-161, 184-188;
-//                                     transformers Qwen2RMSNorm (modeling_qwen2.py:249-266)
-//   gemv epilogues SWIGLU/GATED_RESID modular_vibevoice_diffusion_head.py:116-123, 158-161
+//   gemv prologue RMSNORM             modular_vibevoice_tokenizer.py:53-72 (Block1D ffn_norm, 676);
+//                                     modeling_vibevoice.py:58-69 (SpeechConnector norm, transformers LlamaRMSNorm)
 //   gemv epilogues GELU/GAMMA_RESID   modular_vibevoice_tokenizer.py:592-596, 670-682
+//   gemv epilogue SILU                modular_vibevoice_diffusion_head.py:58-63 (TimestepEmbedder mlp)
 //   assemble_window / dwconv_res      modular_vibevoice_tokenizer.py:327-382 (streaming SConv1d), 786-794
 // (decode attention and the DPM-Solver++ update run only inside the weight-stream kernel: anchors at SAtt / SDpm in vv_stream.cuh)
 #pragma once
@@ -24,8 +24,8 @@ namespace vv {
 
 typedef __nv_bfloat16 bf16;
 
-enum Prologue { PRO_NONE = 0, PRO_RMSNORM = 1, PRO_ADALN = 2, PRO_SILU = 3 };
-enum Epilogue { EPI_NONE = 0, EPI_RESID = 2, EPI_GATED_RESID = 3, EPI_GAMMA_RESID = 4, EPI_SWIGLU = 5, EPI_GELU = 6, EPI_SILU = 7 };
+enum Prologue { PRO_NONE = 0, PRO_RMSNORM = 1 };
+enum Epilogue { EPI_NONE = 0, EPI_RESID = 2, EPI_GAMMA_RESID = 4, EPI_GELU = 6, EPI_SILU = 7 };
 
 // row m of a logical [M, K] operand lives at base + (m / T) * bs + (m % T) * rs; rows may overlap
 // (rs < K) -- that is how causal / strided / transposed convolutions read their input window.
@@ -47,14 +47,10 @@ struct GemvP {
   int ldy;
   int M, N, K;
   int pro;
-  const float* pro_w;       // [K] norm weight (may be null for ADALN without affine)
+  const float* pro_w;       // [K] norm weight
   float pro_eps;
-  const float* pro_shift;   // ADALN: [M, pro_ld]
-  const float* pro_scale;
-  long long pro_ld;
   int epi;
-  const float* epi_a;       // GATED_RESID: gate [M, epi_lda]; GAMMA_RESID: gamma [N]
-  long long epi_lda;
+  const float* epi_a;       // GAMMA_RESID: gamma [N]
   const float* res;         // residual [M, ldres]
   int ldres;
   int WK;                   // warps splitting K inside a CTA (1,2,4,8); WR = 8 / WK row-quads per task
@@ -106,7 +102,6 @@ VV_DEVINL void epi_store_e(const GemvP& p, int epi, int m, int n, float v) {
   // n indexes the weight row; bias already added; `epi` may be a compile-time constant at the call site
   switch (epi) {
     case EPI_RESID: v += p.res[(long long)m * p.ldres + n]; break;
-    case EPI_GATED_RESID: v = p.res[(long long)m * p.ldres + n] + p.epi_a[(long long)m * p.epi_lda + n] * v; break;
     case EPI_GAMMA_RESID: v = p.res[(long long)m * p.ldres + n] + p.epi_a[n] * v; break;
     case EPI_GELU: v = gelu_erf_f(v); break;
     case EPI_SILU: v = silu_f(v); break;
@@ -168,7 +163,7 @@ __global__ void __launch_bounds__(256) gemv_kernel(GemvP p) {
     }
     pdl_wait();                            // predecessor's activations are complete and visible from here on
     // ---- stage pro(x) for rows m0..m0+MB-1: one pass over x (values parked in registers across the norm reduction) ----
-    const bool need_inv = (p.pro == PRO_RMSNORM || p.pro == PRO_ADALN);
+    const bool need_inv = (p.pro == PRO_RMSNORM);
     const int K4 = K >> 2;
     constexpr int XR = 4;                  // float4 per thread per row kept in registers (covers K <= 4096)
     const bool one_pass = (K4 <= XR * 256);
@@ -203,16 +198,6 @@ __global__ void __launch_bounds__(256) gemv_kernel(GemvP p) {
           if (p.pro == PRO_RMSNORM) {
             const float4 w = *reinterpret_cast<const float4*>(p.pro_w + k);
             v.x *= inv * w.x; v.y *= inv * w.y; v.z *= inv * w.z; v.w *= inv * w.w;
-          } else if (p.pro == PRO_ADALN) {
-            float4 w = make_float4(1.f, 1.f, 1.f, 1.f);
-            if (p.pro_w) w = *reinterpret_cast<const float4*>(p.pro_w + k);
-            const long long o = (long long)(m0 + m) * p.pro_ld + k;
-            const float4 sc = *reinterpret_cast<const float4*>(p.pro_scale + o);
-            const float4 sh = *reinterpret_cast<const float4*>(p.pro_shift + o);
-            v.x = v.x * inv * w.x * (1.f + sc.x) + sh.x; v.y = v.y * inv * w.y * (1.f + sc.y) + sh.y;
-            v.z = v.z * inv * w.z * (1.f + sc.z) + sh.z; v.w = v.w * inv * w.w * (1.f + sc.w) + sh.w;
-          } else if (p.pro == PRO_SILU) {
-            v.x = silu_f(v.x); v.y = silu_f(v.y); v.z = silu_f(v.z); v.w = silu_f(v.w);
           }
         } else {
           v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -235,16 +220,15 @@ __global__ void __launch_bounds__(256) gemv_kernel(GemvP p) {
       for (int r = 0; r < 4; ++r)
 #pragma unroll
         for (int m = 0; m < MB; ++m) acc[r][m] = 0.f;
-      // residual / gate operands of this task's outputs are requested now, consumed after the reduction
+      // residual / gamma operands of this task's outputs are requested now, consumed after the reduction
       float pre_res = 0.f, pre_gate = 1.f;
-      const bool has_res = (p.epi == EPI_RESID || p.epi == EPI_GATED_RESID || p.epi == EPI_GAMMA_RESID);
+      const bool has_res = (p.epi == EPI_RESID || p.epi == EPI_GAMMA_RESID);
       if (has_res && tid < WR * 4 * MB) {
         const int q = tid / (4 * MB), r = (tid / MB) % 4, m = tid % MB;
         const int n = (task * WR + q) * 4 + r;
         if (n < N && m0 + m < p.M) {
           pre_res = p.res[(long long)(m0 + m) * p.ldres + n];
-          if (p.epi == EPI_GATED_RESID) pre_gate = p.epi_a[(long long)(m0 + m) * p.epi_lda + n];
-          else if (p.epi == EPI_GAMMA_RESID) pre_gate = p.epi_a[n];
+          if (p.epi == EPI_GAMMA_RESID) pre_gate = p.epi_a[n];
         }
       }
       while (c < nchunks) {
@@ -294,33 +278,17 @@ __global__ void __launch_bounds__(256) gemv_kernel(GemvP p) {
       }
       __syncthreads();
       // ---- epilogue: one thread per (row-quad, r, m) ----
-      if (p.epi == EPI_SWIGLU) {
-        if (tid < WR * 2 * MB) {
-          const int q = tid / (2 * MB), pr = (tid / MB) % 2, m = tid % MB;
-          const int n0 = (this_task * WR + q) * 4 + pr * 2;
-          if (n0 + 1 < N && m0 + m < p.M) {
-            float g = 0.f, u = 0.f;
-            for (int s = 0; s < WK; ++s) {
-              g += rbuf[(q * WK + s) * (4 * MB) + (pr * 2) * MB + m];
-              u += rbuf[(q * WK + s) * (4 * MB) + (pr * 2 + 1) * MB + m];
-            }
-            if (p.bias) { g += p.bias[n0]; u += p.bias[n0 + 1]; }
-            p.y[(long long)(m0 + m) * p.ldy + (n0 >> 1)] = silu_f(g) * u;
-          }
-        }
-      } else {
-        if (tid < WR * 4 * MB) {
-          const int q = tid / (4 * MB), r = (tid / MB) % 4, m = tid % MB;
-          const int n = (this_task * WR + q) * 4 + r;
-          if (n < N && m0 + m < p.M) {
-            float v = 0.f;
-            for (int s = 0; s < WK; ++s) v += rbuf[(q * WK + s) * (4 * MB) + r * MB + m];
-            if (p.bias) v += p.bias[n];
-            if (has_res) v = pre_res + pre_gate * v;
-            else if (p.epi == EPI_GELU) v = gelu_erf_f(v);
-            else if (p.epi == EPI_SILU) v = silu_f(v);
-            p.y[(long long)(m0 + m) * p.ldy + n] = v;
-          }
+      if (tid < WR * 4 * MB) {
+        const int q = tid / (4 * MB), r = (tid / MB) % 4, m = tid % MB;
+        const int n = (this_task * WR + q) * 4 + r;
+        if (n < N && m0 + m < p.M) {
+          float v = 0.f;
+          for (int s = 0; s < WK; ++s) v += rbuf[(q * WK + s) * (4 * MB) + r * MB + m];
+          if (p.bias) v += p.bias[n];
+          if (has_res) v = pre_res + pre_gate * v;
+          else if (p.epi == EPI_GELU) v = gelu_erf_f(v);
+          else if (p.epi == EPI_SILU) v = silu_f(v);
+          p.y[(long long)(m0 + m) * p.ldy + n] = v;
         }
       }
       parity ^= 1;
@@ -358,12 +326,14 @@ VV_DEVINL void bulk_g2s(void* smem_dst, const void* gsrc, unsigned bytes, unsign
 VV_DEVINL void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
-// Tensor-core GEMM for the codec stages with many rows (M > 8): C[M,N] = A[M,K] * W[N,K]^T.
-// A is fp32 in global memory and is split on the fly into bf16 hi + bf16 lo (A = hi + lo up to
-// 2^-16 relative), W is bf16, so two bf16 MMAs per tile reproduce the fp32-activation result of
-// the GEMV path to ~1e-5 while running on the tensor pipe.  CTA tile 32 x 64 x 64, 4 warps, W
-// streamed with a 3-stage cp.async ring, A register-prefetched one k-step ahead.
-// (mma.sync m16n8k16.)
+// Tensor-core GEMM for the codec GEMMs with M > 8 (FFNs, transposed convs): C[M,N] = epi(pro(A)[M,K] * W[N,K]^T), prologue none or RMSNorm.
+// A is fp32 in global memory and is split on the fly into bf16 hi + bf16 lo (A = hi + lo up to 2^-16 relative), W is bf16, so two bf16
+// MMAs per tile reproduce the fp32-activation result of the GEMV path to ~1e-5 while running on the tensor pipe.  CTA tile 32 x 64 x 64,
+// 4 warps (warp = 16 output columns), mma.sync m16n8k16.
+// These GEMMs are tiny (K = 32..2048, <= 112 CTAs), so a CTA must not pay one L2/DRAM round trip per k-step: BOTH operands arrive by
+// cp.async into a 6-stage ring -- fp32 A tile [32 x 64] and bf16 W tile [64 x 64] per stage -- so up to five k-steps (usually the whole K
+// of a split) are in flight from the first instruction and a CTA pays ~one round trip in total.  The fp32 A tile is converted to the bf16
+// hi/lo mma fragments straight from shared memory (LDS.64 per fragment register, row stride 72 floats = conflict-free).
 // ---------------------------------------------------------------------------------------------
 VV_DEVINL void cp_async16(void* smem, const void* gmem, int src_bytes) {
   unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
@@ -384,149 +354,7 @@ VV_DEVINL unsigned pack_bf16(float lo, float hi) {
   return *reinterpret_cast<unsigned*>(&v);
 }
 
-constexpr int MM_BM = 32, MM_BN = 64, MM_BK = 64, MM_ST = 3, MM_LD = MM_BK + 8;   // +8 bf16 = 16 B row pad (ldmatrix conflict-free)
-__global__ void __launch_bounds__(128) gemm_mma_kernel(GemvP p) {
-  __shared__ __align__(16) bf16 Ah[MM_BM][MM_LD];
-  __shared__ __align__(16) bf16 Al[MM_BM][MM_LD];
-  __shared__ __align__(16) bf16 Ws[MM_ST][MM_BN][MM_LD];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int bm = blockIdx.y * MM_BM, bn = blockIdx.x * MM_BN;
-  const int K = p.K, nk_all = (K + MM_BK - 1) / MM_BK;
-  // split-K (gridDim.z > 1): only launched for in-place residual epilogues (y == res); each split atomically adds its
-  // scaled partial into y, split 0 also adds the bias.  Few-CTA, long-K shapes (codec FFN2) get z-times the parallelism.
-  const int kz = blockIdx.z, nz = gridDim.z;
-  const int kt0 = (int)(((long long)nk_all * kz) / nz), kt1 = (int)(((long long)nk_all * (kz + 1)) / nz);
-  const int nk = kt1 - kt0;
-  // A loader: thread -> row tid/4, 16 consecutive k at (tid%4)*16
-  const int ar = tid >> 2, ac = (tid & 3) * 16;
-  const float* arow = (bm + ar < p.M) ? p.x + p.xmap.off(bm + ar) : nullptr;
-  // W loader: 64 rows x 64 k bf16 = 512 x 16 B; thread handles 4 of them
-  auto load_w = [&](int stage, int kt) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int idx = tid + i * 128, r = idx >> 3, c = (idx & 7) * 8;
-      const int n = bn + r, k = (kt0 + kt) * MM_BK + c;
-      const bool ok = (n < p.N) && (k < K);
-      cp_async16(&Ws[stage][r][c], p.W + (size_t)(ok ? n : 0) * K + (ok ? k : 0), ok ? 16 : 0);
-    }
-  };
-  float4 areg[4];
-  float a_inv = 1.f;            // PRO_RMSNORM: row scale, applied together with the norm weight while converting A
-  auto load_a = [&](int kt) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int k = (kt0 + kt) * MM_BK + ac + i * 4;
-      areg[i] = (arow && k < K) ? *reinterpret_cast<const float4*>(arow + k) : make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p.pro == PRO_RMSNORM && arow && k < K) {
-        const float4 wv = *reinterpret_cast<const float4*>(p.pro_w + k);
-        areg[i].x *= a_inv * wv.x; areg[i].y *= a_inv * wv.y; areg[i].z *= a_inv * wv.z; areg[i].w *= a_inv * wv.w;
-      } else if (p.pro == PRO_ADALN && arow && k < K) {
-        float4 wv = make_float4(1.f, 1.f, 1.f, 1.f);
-        if (p.pro_w) wv = *reinterpret_cast<const float4*>(p.pro_w + k);
-        const long long o = (long long)(bm + ar) * p.pro_ld + k;
-        const float4 sc = *reinterpret_cast<const float4*>(p.pro_scale + o);
-        const float4 sh = *reinterpret_cast<const float4*>(p.pro_shift + o);
-        areg[i].x = areg[i].x * a_inv * wv.x * (1.f + sc.x) + sh.x; areg[i].y = areg[i].y * a_inv * wv.y * (1.f + sc.y) + sh.y;
-        areg[i].z = areg[i].z * a_inv * wv.z * (1.f + sc.z) + sh.z; areg[i].w = areg[i].w * a_inv * wv.w * (1.f + sc.w) + sh.w;
-      } else if (p.pro == PRO_SILU && arow && k < K) {
-        areg[i].x = silu_f(areg[i].x); areg[i].y = silu_f(areg[i].y); areg[i].z = silu_f(areg[i].z); areg[i].w = silu_f(areg[i].w);
-      }
-    }
-  };
-  auto store_a = [&]() {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float v[4] = {areg[i].x, areg[i].y, areg[i].z, areg[i].w};
-      float h[4], l[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { h[j] = __bfloat162float(__float2bfloat16_rn(v[j])); l[j] = v[j] - h[j]; }
-      *reinterpret_cast<uint2*>(&Ah[ar][ac + i * 4]) = make_uint2(pack_bf16(h[0], h[1]), pack_bf16(h[2], h[3]));
-      *reinterpret_cast<uint2*>(&Al[ar][ac + i * 4]) = make_uint2(pack_bf16(l[0], l[1]), pack_bf16(l[2], l[3]));
-    }
-  };
-  float acc[2][2][4];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.f;
-
-  pdl_trigger();
-#pragma unroll
-  for (int s_ = 0; s_ < MM_ST - 1; ++s_) { if (s_ < nk) load_w(s_, s_); cp_async_commit(); }
-  pdl_wait();
-  if (p.pro == PRO_RMSNORM || p.pro == PRO_ADALN) {   // 4 threads share a row: each sums a quarter of it, combined with two shuffles
-    float ss = 0.f;
-    if (arow) for (int k = (tid & 3) * 4; k < K; k += 16) { const float4 v = *reinterpret_cast<const float4*>(arow + k); ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w; }
-    ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-    ss += __shfl_xor_sync(0xffffffffu, ss, 2);
-    a_inv = rsqrtf(ss / (float)K + p.pro_eps);
-  }
-  load_a(0);
-  for (int kt = 0; kt < nk; ++kt) {
-    __syncthreads();                       // previous step's readers of Ah/Al and of the stage about to be refilled are done
-    store_a();
-    if (kt + MM_ST - 1 < nk) load_w((kt + MM_ST - 1) % MM_ST, kt + MM_ST - 1);
-    cp_async_commit();
-    if (kt + 1 < nk) load_a(kt + 1);
-    cp_async_wait<MM_ST - 1>();            // stage kt has landed
-    __syncthreads();
-    const int st = kt % MM_ST;
-#pragma unroll
-    for (int kk = 0; kk < MM_BK; kk += 16) {
-      unsigned ah[2][4], al[2][4], bw[4];
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        ldmatrix_x4(ah[mt], &Ah[mt * 16 + (lane & 15)][kk + (lane >> 4) * 8]);
-        ldmatrix_x4(al[mt], &Al[mt * 16 + (lane & 15)][kk + (lane >> 4) * 8]);
-      }
-      // B fragments for this warp's two n-tiles (16 rows of W): lanes 0-7 n0..7 @k, 8-15 n0..7 @k+8, 16-23 n8..15 @k, 24-31 n8..15 @k+8
-      ldmatrix_x4(bw, &Ws[st][warp * 16 + (lane & 7) + ((lane >> 4) << 3)][kk + ((lane >> 3) & 1) * 8]);
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        mma_bf16_16816(acc[mt][0], ah[mt], bw[0], bw[1]);
-        mma_bf16_16816(acc[mt][0], al[mt], bw[0], bw[1]);
-        mma_bf16_16816(acc[mt][1], ah[mt], bw[2], bw[3]);
-        mma_bf16_16816(acc[mt][1], al[mt], bw[2], bw[3]);
-      }
-    }
-  }
-#pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-    for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int m = bm + mt * 16 + (lane >> 2) + (q >> 1) * 8;
-        const int n = bn + warp * 16 + nt * 8 + (lane & 3) * 2 + (q & 1);
-        if (p.epi == EPI_SWIGLU) {                 // (gate, up) = (even, odd) weight rows = (c0,c1) / (c2,c3) of one thread
-          if ((q & 1) == 0 && m < p.M && n + 1 < p.N) {
-            const float g_ = acc[mt][nt][q] + (p.bias ? p.bias[n] : 0.f), u_ = acc[mt][nt][q + 1] + (p.bias ? p.bias[n + 1] : 0.f);
-            p.y[(long long)m * p.ldy + (n >> 1)] = silu_f(g_) * u_;
-          }
-        } else if (m < p.M && n < p.N) {
-          if (nz == 1) {
-            epi_store(p, m, n, acc[mt][nt][q] + (p.bias ? p.bias[n] : 0.f));
-          } else {
-            float v = acc[mt][nt][q] + ((kz == 0 && p.bias) ? p.bias[n] : 0.f);
-            if (p.epi == EPI_GAMMA_RESID) v *= p.epi_a[n];
-            else if (p.epi == EPI_GATED_RESID) v *= p.epi_a[(long long)m * p.epi_lda + n];
-            atomicAdd(p.y + (long long)m * p.ldy + n, v);
-          }
-        }
-      }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Deep-ring variant of gemm_mma_kernel for the codec GEMMs with M > 8 (FFNs, transposed convs); prologue none or RMSNorm.
-// Why: these GEMMs are tiny (K = 32..2048, <= 112 CTAs) and each CTA used to pay one L2/DRAM round trip PER k-step
-// (A register-prefetched one step ahead, W two steps ahead).  Here BOTH operands arrive by cp.async into a 6-stage ring -- fp32 A tile [32 x 64] and bf16 W tile [64 x 64] per stage --
-// so up to five k-steps (usually the whole K of a split) are in flight from the first instruction and a CTA pays ~one round trip in
-// total.  The fp32 A tile is converted to the bf16 hi/lo mma fragments straight from shared memory (LDS.64 per fragment register,
-// row stride 72 floats = conflict-free), which also removes the second __syncthreads and the Ah/Al staging of the old kernel.
-// Same tile (32 x 64 x 64, 4 warps, warp = 16 output columns), same split-K / epilogue semantics, same hi+lo accuracy.
-// ---------------------------------------------------------------------------------------------
+constexpr int MM_BM = 32, MM_BN = 64, MM_BK = 64, MM_LD = MM_BK + 8;   // +8 bf16 = 16 B row pad (ldmatrix conflict-free)
 constexpr int MR_ST = 6, MR_ALD = MM_BK + 8;   // 72-float rows: a half-warp LDS.64 (4 rows x 8 words) hits 32 distinct banks
 constexpr int MR_A_BYTES = MM_BM * MR_ALD * 4, MR_W_BYTES = MM_BN * MM_LD * 2, MR_STAGE = MR_A_BYTES + MR_W_BYTES;
 constexpr int MR_SMEM = MR_ST * MR_STAGE;
@@ -540,6 +368,8 @@ __global__ void __launch_bounds__(128) gemm_mma_ring_kernel(GemvP p) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int bm = blockIdx.y * MM_BM, bn = blockIdx.x * MM_BN;
   const int K = p.K, nk_all = (K + MM_BK - 1) / MM_BK;
+  // split-K (gridDim.z > 1): only launched for in-place residual epilogues (y == res); each split atomically adds its
+  // scaled partial into y, split 0 also adds the bias.  Few-CTA, long-K shapes (codec FFN2) get z-times the parallelism.
   const int kz = blockIdx.z, nz = gridDim.z;
   const int kt0 = (int)(((long long)nk_all * kz) / nz), kt1 = (int)(((long long)nk_all * (kz + 1)) / nz);
   const int nk = kt1 - kt0;
@@ -654,7 +484,6 @@ __global__ void __launch_bounds__(128) gemm_mma_ring_kernel(GemvP p) {
           } else {
             float v = acc[mt][nt][q] + ((kz == 0 && p.bias) ? p.bias[n] : 0.f);
             if (epi == EPI_GAMMA_RESID) v *= p.epi_a[n];
-            else if (epi == EPI_GATED_RESID) v *= p.epi_a[(long long)m * p.epi_lda + n];
             atomicAdd(p.y + (long long)m * p.ldy + n, v);
           }
         }

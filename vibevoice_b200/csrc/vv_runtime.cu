@@ -98,9 +98,6 @@ struct vv_ctx {
   bool use_pdl = true;
   bf16* s_planes = nullptr; size_t planes_elems = 0;
   int use_wgmma = 1;        // warpgroup (wgmma) GEMM: 0 off, 1 auto (wide GEMMs), 2 every M > 8 GEMM (VV_WGMMA)
-  int wr_tasks_min = 296;
-  int wr_force = 0;
-  int gemv_grid_cap = 0;
   int sm_count = 132;
   std::map<std::string, RawTensor> raw;
   std::set<std::string> expected;
@@ -201,8 +198,6 @@ static int gemv_smem_bytes(int MB, int K) { int Kp = (K + 255) & ~255; return (M
 
 template <int MB>
 static int launch_gemv_t(const L& l, GemvP& p, int grid, int smem) {
-  static bool attr_set[8] = {false, false, false, false, false, false, false, false};
-  (void)attr_set;
   CK(cudaFuncSetAttribute(gemv_kernel<MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   CK(launch_k(l, gemv_kernel<MB>, dim3(grid), dim3(256), smem, p));
   return 0;
@@ -220,20 +215,23 @@ static int gemv_occupancy(vv_ctx* c, int smem) {
   return occ;
 }
 
-// which kernel linear() ran (vv_debug_gemv2)
+// which kernel linear() ran (vv_debug_gemv2); 8 is retired
 enum {
   LIN_GEMV = 0, LIN_RING_RMS_GELU, LIN_RING_RMS_NONE, LIN_RING_GAMMA_RESID, LIN_RING_NONE, LIN_RING_GELU, LIN_RING_RESID, LIN_RING_GENERIC,
-  LIN_MMA, LIN_WGMMA
+  LIN_WGMMA = 9
 };
 
-// y = epi(W * pro(x) + bias); dispatches GEMV (M <= 16) or the tiled GEMM.  info (optional): {LIN_* kernel, split-K factor}.
+// y = epi(W * pro(x) + bias); dispatches GEMV (M <= 8) or the tiled GEMM.  info (optional): {LIN_* kernel, split-K factor}.
 static int linear(const L& l, GemvP p, int32_t* info = nullptr) {
   if (p.K % 8 != 0) return fail(VV_ERR_INVALID, "linear: K=%d not a multiple of 8", p.K);
   if (((uintptr_t)p.x & 15) || (p.xmap.rs & 3) || (p.xmap.bs & 3)) return fail(VV_ERR_INVALID, "linear: activation rows must be 16-byte aligned");
+  if (p.pro != PRO_NONE && p.pro != PRO_RMSNORM) return fail(VV_ERR_INVALID, "linear: prologue %d has no kernel", p.pro);
+  if (p.epi != EPI_NONE && p.epi != EPI_RESID && p.epi != EPI_GAMMA_RESID && p.epi != EPI_GELU && p.epi != EPI_SILU)
+    return fail(VV_ERR_INVALID, "linear: epilogue %d has no kernel", p.epi);
   // wgmma path: wide GEMMs that fill the chip with 128-row weight tiles (the all-steps AdaLN modulation GEMM:
   // [N_steps*2B, H] x [(3L+2)H, H]^T = 168 CTAs on 1.5B); mode 2 forces it for every M > 8 GEMM (tests)
   const int wg_ctas = ((p.N + WG_BM - 1) / WG_BM) * ((p.M + WG_BN - 1) / WG_BN);
-  if (l.c->use_wgmma && p.M > 8 && p.pro == PRO_NONE && p.epi != EPI_SWIGLU && (l.c->use_wgmma == 2 || wg_ctas >= 96)) {
+  if (l.c->use_wgmma && p.M > 8 && p.pro == PRO_NONE && (l.c->use_wgmma == 2 || wg_ctas >= 96)) {
     if ((size_t)p.M * p.K > l.c->planes_elems) return fail(VV_ERR_INVALID, "wgmma: activation planes scratch too small (%d x %d)", p.M, p.K);
     bf16* hi = l.c->s_planes;
     bf16* lo = l.c->s_planes + l.c->planes_elems;
@@ -246,48 +244,44 @@ static int linear(const L& l, GemvP p, int32_t* info = nullptr) {
   }
   if (p.M >= MMA_MIN_ROWS) {
     dim3 grid((p.N + MM_BN - 1) / MM_BN, (p.M + MM_BM - 1) / MM_BM);
-    const bool inplace_res = (p.epi == EPI_RESID || p.epi == EPI_GAMMA_RESID || p.epi == EPI_GATED_RESID) && p.res == p.y && p.ldres == p.ldy;
+    const bool inplace_res = (p.epi == EPI_RESID || p.epi == EPI_GAMMA_RESID) && p.res == p.y && p.ldres == p.ldy;
     const int nk = (p.K + MM_BK - 1) / MM_BK;
     if (inplace_res && nk >= 8 && (int)(grid.x * grid.y) < l.c->sm_count) {
       int z = std::min(std::min(nk / 2, 16), (2 * l.c->sm_count) / (int)(grid.x * grid.y));
       grid.z = std::max(z, 1);
     }
     const bool ring_rms = p.pro == PRO_RMSNORM && grid.z == 1 && p.K <= MR_MAXK_NORM && p.K % 4 == 0;
-    if ((p.pro == PRO_NONE || ring_rms) && p.epi != EPI_SWIGLU) {
-      // the combinations the codec passes use get their own instantiation (FFN1: folded RMSNorm + GELU; FFN2 / transposed convs: plain or
-      // gamma-residual, split-K or not); anything else runs the run-time-switched one
-      void (*fn)(GemvP) = gemm_mma_ring_kernel<-1, -1>;
-      int which = LIN_RING_GENERIC;
-      if (ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<1, EPI_GELU>, which = LIN_RING_RMS_GELU;
-      else if (ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<1, EPI_NONE>, which = LIN_RING_RMS_NONE;
-      else if (!ring_rms && p.epi == EPI_GAMMA_RESID) fn = gemm_mma_ring_kernel<0, EPI_GAMMA_RESID>, which = LIN_RING_GAMMA_RESID;
-      else if (!ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<0, EPI_NONE>, which = LIN_RING_NONE;
-      else if (!ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<0, EPI_GELU>, which = LIN_RING_GELU;
-      else if (!ring_rms && p.epi == EPI_RESID) fn = gemm_mma_ring_kernel<0, EPI_RESID>, which = LIN_RING_RESID;
-      CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MR_SMEM_NORM));
-      CK(launch_k(l, fn, dim3(grid), dim3(128), (size_t)(ring_rms ? MR_SMEM_NORM : MR_SMEM), p));
-      if (info) { info[0] = which; info[1] = (int32_t)grid.z; }
-      return 0;
-    }
-    CK(launch_k(l, gemm_mma_kernel, dim3(grid), dim3(128), 0, p));
-    if (info) { info[0] = LIN_MMA; info[1] = (int32_t)grid.z; }
+    if (p.pro == PRO_RMSNORM && !ring_rms)
+      return fail(VV_ERR_INVALID, "linear: RMSNorm at M=%d needs K <= %d, K %% 4 == 0 and no K split (K=%d, split %u)", p.M, MR_MAXK_NORM, p.K,
+                  grid.z);
+    // the combinations the codec passes use get their own instantiation (FFN1: folded RMSNorm + GELU; FFN2 / transposed convs: plain or
+    // gamma-residual, split-K or not); anything else runs the run-time-switched one
+    void (*fn)(GemvP) = gemm_mma_ring_kernel<-1, -1>;
+    int which = LIN_RING_GENERIC;
+    if (ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<1, EPI_GELU>, which = LIN_RING_RMS_GELU;
+    else if (ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<1, EPI_NONE>, which = LIN_RING_RMS_NONE;
+    else if (!ring_rms && p.epi == EPI_GAMMA_RESID) fn = gemm_mma_ring_kernel<0, EPI_GAMMA_RESID>, which = LIN_RING_GAMMA_RESID;
+    else if (!ring_rms && p.epi == EPI_NONE) fn = gemm_mma_ring_kernel<0, EPI_NONE>, which = LIN_RING_NONE;
+    else if (!ring_rms && p.epi == EPI_GELU) fn = gemm_mma_ring_kernel<0, EPI_GELU>, which = LIN_RING_GELU;
+    else if (!ring_rms && p.epi == EPI_RESID) fn = gemm_mma_ring_kernel<0, EPI_RESID>, which = LIN_RING_RESID;
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MR_SMEM_NORM));
+    CK(launch_k(l, fn, dim3(grid), dim3(128), (size_t)(ring_rms ? MR_SMEM_NORM : MR_SMEM), p));
+    if (info) { info[0] = which; info[1] = (int32_t)grid.z; }
     return 0;
   }
   int MB = p.M <= 1 ? 1 : (p.M <= 2 ? 2 : (p.M <= 4 ? 4 : 8));
   while (MB > 1 && gemv_smem_bytes(MB, p.K) > 200 * 1024) MB >>= 1;
   if (gemv_smem_bytes(MB, p.K) > 200 * 1024) return fail(VV_ERR_INVALID, "gemv: K=%d too large", p.K);
   int WR = 8;
-  while (WR > 1 && (p.N + 4 * WR - 1) / (4 * WR) < l.c->wr_tasks_min) WR >>= 1;
+  while (WR > 1 && (p.N + 4 * WR - 1) / (4 * WR) < l.c->sm_count) WR >>= 1;   // at least one task per SM
   const int nchunks = (p.K + 255) / 256;
   while (WR < 8 && 8 / WR > nchunks) WR <<= 1;      // never more k-split warps than 256-element chunks
-  if (l.c->wr_force) WR = l.c->wr_force;
   p.WK = 8 / WR;
   const int ntasks = (p.N + 4 * WR - 1) / (4 * WR);
   const int smem = gemv_smem_bytes(MB, p.K);
   int occ = MB == 1 ? gemv_occupancy<1>(l.c, smem) : MB == 2 ? gemv_occupancy<2>(l.c, smem) : MB == 4 ? gemv_occupancy<4>(l.c, smem)
                                                                                                           : gemv_occupancy<8>(l.c, smem);
-  int grid = std::min(ntasks, l.c->sm_count * occ);
-  if (l.c->gemv_grid_cap) grid = std::min(grid, l.c->gemv_grid_cap);
+  const int grid = std::min(ntasks, l.c->sm_count * occ);
   if (info) { info[0] = LIN_GEMV; info[1] = 1; }
   switch (MB) {
     case 1: return launch_gemv_t<1>(l, p, grid, smem);
@@ -704,10 +698,6 @@ extern "C" int vv_create(const vv_model_desc* desc, int device, vv_ctx** out) {
   c->sm_count = prop.multiProcessorCount;
   const char* ng = getenv("VV_NO_GRAPH");
   c->use_graphs = !(ng && ng[0] == '1');
-  c->wr_tasks_min = c->sm_count;      // one task per SM (tools/bench_gemv.py compares geometries)
-  if (getenv("VV_WR_TASKS_MIN")) c->wr_tasks_min = atoi(getenv("VV_WR_TASKS_MIN"));
-  if (getenv("VV_WR_FORCE")) c->wr_force = atoi(getenv("VV_WR_FORCE"));
-  if (getenv("VV_GEMV_GRID_CAP")) c->gemv_grid_cap = atoi(getenv("VV_GEMV_GRID_CAP"));
   if (getenv("VV_STREAM_INFLIGHT")) c->st_inflight = atoi(getenv("VV_STREAM_INFLIGHT"));
   if (getenv("VV_WGMMA")) c->use_wgmma = atoi(getenv("VV_WGMMA"));
   const char* np = getenv("VV_NO_PDL");
@@ -2802,30 +2792,16 @@ extern "C" int vv_codec_state_reset(vv_ctx* c, void* stream) {
   return vv_codec_state_zero(c, rows, c->d.max_batch, stream);
 }
 
-extern "C" int vv_debug_gemv(vv_ctx* c, const void* w, const float* bias, const float* x, float* y, int M, int N, int K, int prologue,
-                             const float* pro_w, float eps, int epilogue, void* stream) {
-  if (!c) return fail(VV_ERR_INVALID, "null ctx");
-  CK(cudaSetDevice(c->device));
-  L l{c, (cudaStream_t)stream};
-  const int ldy = epilogue == EPI_SWIGLU ? N / 2 : N;
-  GemvP p = mk((const bf16*)w, bias, x, K, y, ldy, M, N, K);
-  p.pro = prologue; p.pro_w = pro_w; p.pro_eps = eps; p.epi = epilogue;
-  if (epilogue == EPI_RESID) { p.res = y; p.ldres = N; }
-  return linear(l, p);
-}
-
 // linear() with the row map, strides, separate or in-place residual and epilogue operand of the codec's kernel-per-stage GEMMs (see the header)
 extern "C" int vv_debug_gemv2(vv_ctx* c, const void* w, const float* bias, const float* x, int64_t ldx, int map_T, int64_t map_bs, float* y,
                               int64_t ldy, const float* res, int64_t ldres, int M, int N, int K, int prologue, const float* pro_w, float eps,
                               int epilogue, const float* epi_a, int64_t epi_lda, int32_t* info, void* stream) {
+  (void)epi_lda;
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
   if (!w || !x || !y || !info || M < 1 || N < 1 || K < 8) return fail(VV_ERR_INVALID, "vv_debug_gemv2: null operand or empty shape");
-  if (prologue != PRO_NONE && prologue != PRO_RMSNORM && prologue != PRO_SILU) return fail(VV_ERR_INVALID, "vv_debug_gemv2: prologue %d", prologue);
   if (prologue == PRO_RMSNORM && !pro_w) return fail(VV_ERR_INVALID, "vv_debug_gemv2: RMSNorm needs its weight");
-  const bool has_res = epilogue == EPI_RESID || epilogue == EPI_GATED_RESID || epilogue == EPI_GAMMA_RESID;
-  if (epilogue != EPI_NONE && epilogue != EPI_GELU && epilogue != EPI_SILU && !has_res) return fail(VV_ERR_INVALID, "vv_debug_gemv2: epilogue %d", epilogue);
-  if ((has_res && (!res || ldres < N || ldres > INT32_MAX)) || ((epilogue == EPI_GAMMA_RESID || epilogue == EPI_GATED_RESID) && !epi_a) ||
-      (epilogue == EPI_GATED_RESID && epi_lda < N))
+  const bool has_res = epilogue == EPI_RESID || epilogue == EPI_GAMMA_RESID;
+  if ((has_res && (!res || ldres < N || ldres > INT32_MAX)) || (epilogue == EPI_GAMMA_RESID && !epi_a))
     return fail(VV_ERR_INVALID, "vv_debug_gemv2: missing residual / epilogue operand");
   if (ldx < 1 || map_T < 0 || map_bs < 0 || ldy < N || ldy > INT32_MAX) return fail(VV_ERR_INVALID, "vv_debug_gemv2: bad strides");
   CK(cudaSetDevice(c->device));
@@ -2833,7 +2809,7 @@ extern "C" int vv_debug_gemv2(vv_ctx* c, const void* w, const float* bias, const
   GemvP p = mk((const bf16*)w, bias, x, ldx, y, (int)ldy, M, N, K);
   if (map_T > 0) { p.xmap.T = map_T; p.xmap.bs = map_bs; }
   p.pro = prologue; p.pro_w = pro_w; p.pro_eps = eps; p.epi = epilogue;
-  p.epi_a = epi_a; p.epi_lda = epi_lda; p.res = res; p.ldres = (int)ldres;
+  p.epi_a = epi_a; p.res = res; p.ldres = (int)ldres;
   RET(linear(l, p, info));
   CK(cudaStreamSynchronize(l.s));
   CKL();
@@ -2858,22 +2834,7 @@ static int run_debug_stream(vv_ctx* c, StreamBuilder& b, void* stream) {
   return pr.n_ops;
 }
 
-// one linear through the weight-stream kernel (tests): y = [y +] alpha * (W pro(x) + bias); pro = SPro, alpha_kind = SAlpha
-extern "C" int vv_debug_stream_gemv(vv_ctx* c, const void* w, const float* bias, const float* x, float* y, int M, int N, int K, int pro,
-                                    const float* pro_w, float eps, int alpha_kind, const float* alpha, int accumulate, void* stream) {
-  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  CK(cudaSetDevice(c->device));
-  StreamBuilder b(c);
-  b.fresh_weights = true;
-  if (!accumulate) b.nop(false, y, (long long)M * N);
-  SOp* o;
-  RET(b.gemv((const bf16*)w, bias, x, pro == SP_SWIGLU ? 2LL * K : (long long)K, y, N, M, N, K, !accumulate, &o));
-  o->pro = pro; o->pro_w = pro_w; o->pro_eps = eps; o->alpha_kind = alpha_kind; o->alpha = alpha; o->lda = N;
-  const int rc = run_debug_stream(c, b, stream);
-  return rc < 0 ? rc : 0;
-}
-
-// vv_debug_stream_gemv with the strides, AdaLN operands, store epilogue and K split exposed (see the header)
+// one linear through the weight-stream kernel (tests), with the strides, AdaLN operands, store epilogue and K split exposed (see the header)
 extern "C" int vv_debug_stream_gemv2(vv_ctx* c, const void* w, const float* bias, const float* x, int64_t ldx, float* y, int64_t ldy, int M, int N, int K,
                                      int pro, const float* pro_w, float eps, const float* pro_shift, const float* pro_scale, int64_t pro_ld,
                                      int alpha_kind, const float* alpha, int64_t lda, int store, int64_t operand_cap, void* stream) {
