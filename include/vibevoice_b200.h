@@ -145,6 +145,19 @@ int vv_set_step_noise(vv_ctx* ctx, const float* step_noise);
  * latent_out [B,64] fp32 (the *scaled* latent, i.e. what acoustic_connector consumes, :667). */
 int vv_diffusion_sample(vv_ctx* ctx, const float* cond, const float* noise, const int32_t* active, float cfg_scale,
                         float* latent_out, void* stream);
+/* Per-row sampler settings (a request queue mixes step counts, solvers and CFG scales in one batch; demo/gradio_demo.py:141-147, 568
+ * exposes all three per request).  vv_sampler_per_row(n_max > 0) switches the sampler to per-row mode: every row runs n_max solver steps
+ * per frame, and each row starts as n_max identity steps on a zero timestep embedding with CFG scale 1 (its latent is its noise);
+ * n_max = 0 switches back to the global mode of vv_set_diffusion_steps.  Switching drops the captured sampler / frame-tail graphs.
+ * vv_set_row_sampler sets row `row` (< B) to n_steps <= n_max steps: timesteps[n_steps] and coef[n_steps][ncol] as for
+ * vv_set_diffusion_steps (ncol 6, dpmsolver++) or vv_set_diffusion_steps_sde (ncol 7, sde-dpmsolver++), and its CFG scale.  The row runs
+ * n_max - n_steps identity steps conditioned on its first timestep, then its own steps, so its latent is that of a solo run with these
+ * settings.  It writes device memory only: no program is rebuilt and no graph captured.  Step noise for row r's step j lives at
+ * step_noise[n_max - n_steps + j][r] (vv_set_step_noise, [n_max][B][64]), needed once any row is on sde-dpmsolver++.  In per-row mode
+ * vv_diffusion_sample and vv_frame_tail ignore their cfg_scale argument.  Synchronises the stream. */
+int vv_sampler_per_row(vv_ctx* ctx, int n_max, void* stream);
+int vv_set_row_sampler(vv_ctx* ctx, int row, int n_steps, const float* timesteps, const float* coef, int ncol /*6 ODE, 7 SDE*/,
+                       float cfg_scale, void* stream);
 
 /* ---- a-5/a-6/a-7/a-8: codec frame, semantic frame, connectors, streaming state ----------------- */
 int vv_codec_decode_frame(vv_ctx* ctx, const float* latent, const int32_t* active, float* audio_out /*[B,3200]*/, void* stream);

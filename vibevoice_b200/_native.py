@@ -68,6 +68,8 @@ SYMBOLS = {
     "vv_set_diffusion_steps_sde": (_I, [_P, _I, _P, _P, _P]),
     "vv_set_step_noise": (_I, [_P, _P]),
     "vv_diffusion_sample": (_I, [_P, _P, _P, _P, _F, _P, _P]),
+    "vv_sampler_per_row": (_I, [_P, _I, _P]),
+    "vv_set_row_sampler": (_I, [_P, _I, _I, _P, _P, _I, _F, _P]),
     "vv_codec_decode_frame": (_I, [_P, _P, _P, _P, _P]),
     "vv_semantic_encode_frame": (_I, [_P, _P, _P, _P, _P]),
     "vv_connect": (_I, [_P, _P, _P, _P, _P, _P]),

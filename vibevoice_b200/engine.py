@@ -375,6 +375,41 @@ class Engine:
             N.check(self.lib.vv_set_diffusion_steps(self.h, n_steps, N.iptr(ts), N.iptr(coef), self.s), "vv_set_diffusion_steps")
         self.n_steps = n_steps
 
+    def sampler_per_row(self, n_max: int):
+        """Switch the sampler to per-row settings with `n_max` solver steps per frame for every row (`vv_sampler_per_row`); 0 switches back
+        to the global settings of `set_diffusion_steps`, which are then rebuilt on its next call."""
+        n_max = int(n_max)
+        if n_max > 0:
+            with torch.cuda.device(self.device):
+                self.row_step_noise = torch.zeros(n_max, self.B, 64, dtype=torch.float32, device=self.device)
+            N.check(self.lib.vv_set_step_noise(self.h, C.c_void_p(self.row_step_noise.data_ptr())), "vv_set_step_noise")
+        N.check(self.lib.vv_sampler_per_row(self.h, n_max, self.s), "vv_sampler_per_row")
+        self.row_nmax = n_max
+        self.row_steps = [n_max] * self.B
+        if n_max == 0:
+            self.row_step_noise = None
+            self.n_steps = 0                          # the global tables (and step-noise binding) are set again on the next call
+
+    def set_row_sampler(self, row: int, n_steps: int, solver: str, cfg_scale: float):
+        """Row `row` samples with `n_steps` steps of `solver` ("dpmsolver++" or "sde-dpmsolver++", on the engine scheduler's
+        configuration) at CFG scale `cfg_scale` (`vv_set_row_sampler`; device memory only)."""
+        sched = DPMSolverMultistepScheduler.from_config(self.scheduler.config, algorithm_type=solver)
+        sched.set_timesteps(int(n_steps))
+        ts = np.ascontiguousarray(sched.timesteps.numpy().astype(np.float32))
+        coef = np.ascontiguousarray(sched.coef, dtype=np.float32)
+        N.check(self.lib.vv_set_row_sampler(self.h, int(row), int(n_steps), N.iptr(ts), N.iptr(coef), int(coef.shape[1]), float(cfg_scale),
+                                            self.s), "vv_set_row_sampler")
+        self.row_steps[int(row)] = int(n_steps)
+
+    def upload_row_step_noise(self, row: int, noise: torch.Tensor):
+        """sde-dpmsolver++ rows in per-row mode: noise [n_steps, 64] of row `row`'s own steps, which run last of the frame's n_max."""
+        n = self.row_steps[row]
+        with torch.cuda.stream(self.stream):
+            self.row_step_noise[self.row_nmax - n:, row].copy_(noise.to(self.device, torch.float32), non_blocking=True)
+
+    def kv_pages_free(self) -> int:
+        return int(self.lib.vv_kv_pages_free(self.h))
+
     def upload_step_noise(self, draw, active_rows):
         """sde-dpmsolver++: the reference draws randn_tensor([2n,64]) once per solver step on the model's device (dpm_solver.py:993-997)
         and only rows [:n] reach the latent (:703-706); `draw(i)` returns that [2n,64] block for step i."""

@@ -227,12 +227,13 @@ class VibeVoiceForConditionalGenerationInference:
         return self
 
     @torch.no_grad()
-    def _voice_prompt(self, speech_tensors: torch.Tensor, speech_masks: torch.Tensor, scale: float, bias: float, noise=None) -> torch.Tensor:
+    def _voice_prompt(self, speech_tensors: torch.Tensor, speech_masks: torch.Tensor, scale: float, bias: float, noise=None,
+                      generator: Optional[torch.Generator] = None) -> torch.Tensor:
         """Voice-prompt half of step 0 (`modeling_vibevoice_inference.py:149-163, 216-224`) on the engine (`vv_voice_encode`): acoustic
         tokenizer encoder over the padded reference wavs, Gaussian sampling (`modular_vibevoice_tokenizer.py:980-989`), (x + bias) * scale,
         `acoustic_connector`.  -> connected embeddings [sum(speech_masks), H] fp32 on the device, in row-major mask order.  The noise is
-        drawn from the device RNG in the order PyTorch's sampling draws it (std_n [n], then eps [n, F, vae_dim]); `noise=(std_n, eps)`
-        overrides both (tests)."""
+        drawn from the device RNG (or `generator`, a device generator) in the order PyTorch's sampling draws it (std_n [n], then
+        eps [n, F, vae_dim]); `noise=(std_n, eps)` overrides both (tests)."""
         eng = self.engine
         if (float(scale), float(bias)) != (self._scale, self._bias):
             raise ValueError("speech scale / bias (%r, %r) differ from the checkpoint's (%r, %r), which the engine was built with"
@@ -242,11 +243,11 @@ class VibeVoiceForConditionalGenerationInference:
         n, T = wavs.shape
         shape = (n, eng.voice_frames(T), self.config.acoustic_vae_dim)
         if tc.std_dist_type == "gaussian":
-            std_n = torch.randn(n, device=dev) if noise is None else noise[0].to(dev, torch.float32)
-            eps = torch.randn(shape, device=dev) if noise is None else noise[1].to(dev, torch.float32)
+            std_n = torch.randn(n, device=dev, generator=generator) if noise is None else noise[0].to(dev, torch.float32)
+            eps = torch.randn(shape, device=dev, generator=generator) if noise is None else noise[1].to(dev, torch.float32)
             sigma = std_n * (float(tc.fix_std) / 0.8)
         elif tc.std_dist_type == "fix":
-            eps = torch.randn(shape, device=dev) if noise is None else noise[1].to(dev, torch.float32)
+            eps = torch.randn(shape, device=dev, generator=generator) if noise is None else noise[1].to(dev, torch.float32)
             sigma = torch.full((n,), float(tc.fix_std), device=dev)
         else:
             eps, sigma = None, torch.zeros(n, device=dev)
