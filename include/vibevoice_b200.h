@@ -206,12 +206,19 @@ int vv_embed_gather(vv_ctx* ctx, const int32_t* ids_dev, int64_t n, float* out, 
  * Optional weights: model.tts_input_types.weight [2,H], tts_eos_classifier.fc1.{weight [H,H], bias [H]}, fc2.{weight [1,H], bias [1]},
  * all five or none (else vv_finalize_weights fails), kept in fp32 whatever dtype they arrive in; without them both calls return
  * VV_ERR_STATE and vv_weight_bytes(ctx, 6) is 0.
- * vv_tts_type_embed: dst[rows[i]] = src + tts_input_types[type_id] for i < n (n <= 16 host row indices, rows of H fp32 floats; src may be
- * one of them).  One fp32 add per element.
- * vv_eos_prob: prob_out[0] = sigmoid(fc2 . relu(fc1 . hidden + b1) + b2), logit_out[0] (may be NULL) = the logit; hidden [H] fp32, all
- * device pointers.  One launch, fp32 accumulation in a fixed order (results are bit-identical from call to call); calls on one ctx must
- * not overlap (they share a workspace). */
+ * vv_tts_type_embed_rows: dst[dst_rows[i]] = src[src_rows[i]] + tts_input_types[type_ids[i]] for i < n (n <= 16; host arrays of row
+ * indices and types 0 / 1; src and dst are rows of H fp32 floats and may be the same buffer: a source row may also be a destination).
+ * One fp32 add per element, so the result is bit-identical to PyTorch's fp32 add.
+ * vv_tts_type_embed: dst[rows[i]] = src + tts_input_types[type_id] for i < n, i.e. vv_tts_type_embed_rows with every source row 0 of
+ * src and one type (src may be one of the destination rows).
+ * vv_eos_prob_rows: prob_out[i] = sigmoid(fc2 . relu(fc1 . hidden[rows[i]] + b1) + b2), logit_out[i] (may be NULL) = the logit, for
+ * i < n <= 8 (host row indices into hidden [R][H] fp32; device outputs of n floats).  One launch that reads fc1 once for all rows, fp32
+ * accumulation in a fixed order per row: every row's result is bit-identical to vv_eos_prob on that row alone, at any n and position.
+ * vv_eos_prob: vv_eos_prob_rows of the single row hidden [H].  Calls of either on one ctx must not overlap (they share a workspace). */
+int vv_tts_type_embed_rows(vv_ctx* ctx, const float* src, const int32_t* src_rows, const int32_t* type_ids, const int32_t* dst_rows, int n,
+                           float* dst, void* stream);
 int vv_tts_type_embed(vv_ctx* ctx, const float* src, int type_id, const int32_t* rows_host, int n, float* dst, void* stream);
+int vv_eos_prob_rows(vv_ctx* ctx, const float* hidden, const int32_t* rows_host, int n, float* prob_out, float* logit_out, void* stream);
 int vv_eos_prob(vv_ctx* ctx, const float* hidden, float* prob_out, float* logit_out, void* stream);
 
 /* ---- introspection for tests / bench ----------------------------------------------------------- */

@@ -82,7 +82,9 @@ SYMBOLS = {
     "vv_lm_prefill": (_I, [_P, _I, _L, _L, _P, _P, _P, _L, _P]),
     "vv_embed_gather": (_I, [_P, _P, _L, _P, _P]),
     "vv_tts_type_embed": (_I, [_P, _P, _I, _P, _I, _P, _P]),
+    "vv_tts_type_embed_rows": (_I, [_P, _P, _P, _P, _P, _I, _P, _P]),
     "vv_eos_prob": (_I, [_P, _P, _P, _P, _P]),
+    "vv_eos_prob_rows": (_I, [_P, _P, _P, _I, _P, _P, _P]),
     "vv_debug_kv_read": (_I, [_P, _I, _I, _L, _L, _P, _P, _P]),
     "vv_launch_count": (_L, [_P]),
     "vv_debug_barrier_bench": (_I, [_P, _I, _I, C.POINTER(C.c_float)]),

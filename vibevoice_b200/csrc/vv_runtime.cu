@@ -963,7 +963,7 @@ static int build_tts_heads(vv_ctx* c) {
   RET(take_f32(c, "tts_eos_classifier.fc1.bias", {H}, &c->eos_b1, b));
   RET(take_f32(c, "tts_eos_classifier.fc2.weight", {1, H}, &c->eos_w2, b));
   RET(take_f32(c, "tts_eos_classifier.fc2.bias", {1}, &c->eos_b2, b));
-  RET(dmalloc(c, &c->eos_partial, (size_t)(H + EOS_ROWS_PER_CTA - 1) / EOS_ROWS_PER_CTA));
+  RET(dmalloc(c, &c->eos_partial, (size_t)EOS_MAX_ROWS * ((H + EOS_ROWS_PER_CTA - 1) / EOS_ROWS_PER_CTA)));
   RET(dmalloc(c, &c->eos_ticket, 1));
   return 0;
 }
@@ -2814,35 +2814,58 @@ extern "C" int vv_embed_gather(vv_ctx* c, const int32_t* ids_dev, int64_t n, flo
   return 0;
 }
 
-extern "C" int vv_tts_type_embed(vv_ctx* c, const float* src, int type_id, const int32_t* rows_host, int n, float* dst, void* stream) {
+extern "C" int vv_tts_type_embed_rows(vv_ctx* c, const float* src, const int32_t* src_rows, const int32_t* type_ids, const int32_t* dst_rows,
+                                      int n, float* dst, void* stream) {
   if (!c) return fail(VV_ERR_INVALID, "null ctx");
   if (!c->tts_types) return fail(VV_ERR_STATE, "vv_tts_type_embed: no model.tts_input_types loaded");
-  if (!src || !dst || !rows_host) return fail(VV_ERR_INVALID, "vv_tts_type_embed: null argument");
-  if (type_id < 0 || type_id > 1) return fail(VV_ERR_INVALID, "vv_tts_type_embed: type_id %d not 0 or 1", type_id);
+  if (!src || !dst || !src_rows || !type_ids || !dst_rows) return fail(VV_ERR_INVALID, "vv_tts_type_embed: null argument");
   if (n < 1 || n > TTS_MAX_ROWS) return fail(VV_ERR_INVALID, "vv_tts_type_embed: n = %d rows (1..%d)", n, TTS_MAX_ROWS);
   TtsRows rows;
   rows.n = n;
   for (int i = 0; i < n; ++i) {
-    if (rows_host[i] < 0) return fail(VV_ERR_INVALID, "vv_tts_type_embed: negative row %d", rows_host[i]);
+    if (type_ids[i] < 0 || type_ids[i] > 1) return fail(VV_ERR_INVALID, "vv_tts_type_embed: type_id %d not 0 or 1", type_ids[i]);
+    if (dst_rows[i] < 0 || src_rows[i] < 0) return fail(VV_ERR_INVALID, "vv_tts_type_embed: negative row %d / %d", dst_rows[i], src_rows[i]);
+    rows.dst[i] = dst_rows[i];
+    rows.src[i] = src_rows[i];
+    rows.type[i] = type_ids[i];
+  }
+  CK(cudaSetDevice(c->device));
+  const int H = c->d.hidden_size;
+  CK(launch_k(L{c, (cudaStream_t)stream}, tts_type_embed_kernel, dim3((H + 255) / 256), dim3(256), 0, src, (const float*)c->tts_types, rows,
+              dst, H));
+  return 0;
+}
+
+extern "C" int vv_tts_type_embed(vv_ctx* c, const float* src, int type_id, const int32_t* rows_host, int n, float* dst, void* stream) {
+  int32_t zero[TTS_MAX_ROWS] = {}, types[TTS_MAX_ROWS];       // every destination from row 0 of src, with one type
+  for (int i = 0; i < std::min(std::max(n, 0), TTS_MAX_ROWS); ++i) types[i] = type_id;
+  return vv_tts_type_embed_rows(c, src, zero, types, rows_host, n, dst, stream);
+}
+
+extern "C" int vv_eos_prob_rows(vv_ctx* c, const float* hidden, const int32_t* rows_host, int n, float* prob_out, float* logit_out, void* stream) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  if (!c->eos_w1) return fail(VV_ERR_STATE, "vv_eos_prob: no tts_eos_classifier loaded");
+  if (!hidden || !prob_out || !rows_host) return fail(VV_ERR_INVALID, "vv_eos_prob: null argument");
+  if (n < 1 || n > EOS_MAX_ROWS) return fail(VV_ERR_INVALID, "vv_eos_prob_rows: n = %d rows (1..%d)", n, EOS_MAX_ROWS);
+  EosRows rows;
+  rows.n = n;
+  for (int i = 0; i < n; ++i) {
+    if (rows_host[i] < 0) return fail(VV_ERR_INVALID, "vv_eos_prob_rows: negative row %d", rows_host[i]);
     rows.row[i] = rows_host[i];
   }
   CK(cudaSetDevice(c->device));
   const int H = c->d.hidden_size;
-  CK(launch_k(L{c, (cudaStream_t)stream}, tts_type_embed_kernel, dim3((H + 255) / 256), dim3(256), 0, src, (const float*)c->tts_types,
-              type_id, rows, dst, H));
+  const size_t smem = (size_t)n * H * sizeof(float);
+  if (smem > 48 * 1024) CK(cudaFuncSetAttribute(eos_prob_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CK(launch_k(L{c, (cudaStream_t)stream}, eos_prob_kernel, dim3((H + EOS_ROWS_PER_CTA - 1) / EOS_ROWS_PER_CTA), dim3(EOS_THREADS), smem,
+              hidden, rows, (const float*)c->eos_w1, (const float*)c->eos_b1, (const float*)c->eos_w2, (const float*)c->eos_b2, H,
+              c->eos_partial, c->eos_ticket, prob_out, logit_out));
   return 0;
 }
 
 extern "C" int vv_eos_prob(vv_ctx* c, const float* hidden, float* prob_out, float* logit_out, void* stream) {
-  if (!c) return fail(VV_ERR_INVALID, "null ctx");
-  if (!c->eos_w1) return fail(VV_ERR_STATE, "vv_eos_prob: no tts_eos_classifier loaded");
-  if (!hidden || !prob_out) return fail(VV_ERR_INVALID, "vv_eos_prob: null argument");
-  CK(cudaSetDevice(c->device));
-  const int H = c->d.hidden_size;
-  CK(launch_k(L{c, (cudaStream_t)stream}, eos_prob_kernel, dim3((H + EOS_ROWS_PER_CTA - 1) / EOS_ROWS_PER_CTA), dim3(EOS_THREADS),
-              (size_t)H * sizeof(float), hidden, (const float*)c->eos_w1, (const float*)c->eos_b1, (const float*)c->eos_w2,
-              (const float*)c->eos_b2, H, c->eos_partial, c->eos_ticket, prob_out, logit_out));
-  return 0;
+  const int32_t row0 = 0;
+  return vv_eos_prob_rows(c, hidden, &row0, 1, prob_out, logit_out, stream);
 }
 
 extern "C" int vv_debug_kv_read(vv_ctx* c, int seq, int layer, int64_t pos0, int64_t n, void* k_out, void* v_out, void* stream) {

@@ -54,6 +54,8 @@ def _desc_from_config(cfg: VibeVoiceConfig, valid_ids, max_batch: int, max_steps
 class Engine:
     """One GPU's worth of VibeVoice: weights, paged KV, codec state, per-frame programs."""
 
+    EOS_MAX_ROWS = 8                              # hidden rows per vv_eos_prob_rows launch
+
     def __init__(self, config: VibeVoiceConfig, valid_ids, max_batch: int = 1, device: int = 0, max_diffusion_steps: int = 64):
         if not torch.cuda.is_available():
             raise N.VVError("vibevoice_b200 needs a CUDA device (sm_90a); there is no CPU path")
@@ -87,8 +89,8 @@ class Engine:
         self.logits_h = torch.zeros(B, len(self.valid_ids), dtype=torch.float32).pin_memory()
         self.noise_h = torch.zeros(B, 64, dtype=torch.float32).pin_memory()
         self.active_h = torch.zeros(B, dtype=torch.int32).pin_memory()
-        self.eos_d = torch.zeros(2, dtype=torch.float32, device=dev)       # vv_eos_prob: probability, logit
-        self.eos_h = torch.zeros(2, dtype=torch.float32).pin_memory()
+        self.eos_d = torch.zeros(2, self.EOS_MAX_ROWS, dtype=torch.float32, device=dev)     # vv_eos_prob(_rows): probabilities, logits
+        self.eos_h = torch.zeros(2, self.EOS_MAX_ROWS, dtype=torch.float32).pin_memory()
         self.n_steps = 0
         self.step_noise = None
         self.scheduler = DPMSolverMultistepScheduler(
@@ -310,19 +312,53 @@ class Engine:
         N.check(self.lib.vv_tts_type_embed(self.h, C.c_void_p(src.data_ptr()), int(type_id), N.iptr(r), len(r), C.c_void_p(dst.data_ptr()),
                                            self.s), "vv_tts_type_embed")
 
+    def tts_type_embed_rows(self, src: torch.Tensor, src_rows, type_ids, dst_rows, dst: torch.Tensor):
+        """`dst[dst_rows[i]] = src[src_rows[i]] + tts_input_types[type_ids[i]]` for every i (<= 16) in one launch on the engine stream;
+        src [R, H] and dst [R', H] may be the same tensor, and a source row may also be a destination."""
+        for t, what in ((src, "src"), (dst, "dst")):
+            self._row_of(t, what)
+            if t.dim() != 2 or not t.is_contiguous():
+                raise ValueError("%s must be a contiguous [R, H]" % what)
+        sr, ty, dr = N.i32(src_rows), N.i32(type_ids), N.i32(dst_rows)
+        if not len(sr) == len(ty) == len(dr):
+            raise ValueError("src_rows, type_ids and dst_rows differ in length")
+        if any(not 0 <= int(r) < src.shape[0] for r in sr) or any(not 0 <= int(r) < dst.shape[0] for r in dr):
+            raise ValueError("rows outside src's %d / dst's %d rows" % (src.shape[0], dst.shape[0]))
+        N.check(self.lib.vv_tts_type_embed_rows(self.h, C.c_void_p(src.data_ptr()), N.iptr(sr), N.iptr(ty), N.iptr(dr), len(dr),
+                                                C.c_void_p(dst.data_ptr()), self.s), "vv_tts_type_embed_rows")
+
+    def _eos_read(self, n: int):
+        with torch.cuda.stream(self.stream):
+            self.eos_h.copy_(self.eos_d, non_blocking=True)
+        self.stream.synchronize()
+        self.eos_logits = self.eos_h[1, :n].tolist()
+        return self.eos_h[0, :n].tolist()
+
     def eos_prob(self, hidden: Optional[torch.Tensor] = None) -> float:
         """`sigmoid(tts_eos_classifier(hidden))` (default: hidden row 0), synchronising the engine stream; `eos_logit` keeps the logit."""
         h = self.hidden[0] if hidden is None else hidden
         self._row_of(h, "hidden")
         if h.dim() != 1:
             raise ValueError("hidden must be [H]")
-        N.check(self.lib.vv_eos_prob(self.h, C.c_void_p(h.data_ptr()), C.c_void_p(self.eos_d.data_ptr()),
-                                     C.c_void_p(self.eos_d.data_ptr() + 4), self.s), "vv_eos_prob")
-        with torch.cuda.stream(self.stream):
-            self.eos_h.copy_(self.eos_d, non_blocking=True)
-        self.stream.synchronize()
-        self.eos_logit = float(self.eos_h[1])
-        return float(self.eos_h[0])
+        N.check(self.lib.vv_eos_prob(self.h, C.c_void_p(h.data_ptr()), C.c_void_p(self.eos_d[0].data_ptr()),
+                                     C.c_void_p(self.eos_d[1].data_ptr()), self.s), "vv_eos_prob")
+        p = self._eos_read(1)[0]
+        self.eos_logit = self.eos_logits[0]
+        return p
+
+    def eos_probs(self, rows, hidden: Optional[torch.Tensor] = None):
+        """`sigmoid(tts_eos_classifier(hidden[r]))` for every r in `rows` (<= 8; default: the engine's hidden rows) in one launch and one
+        synchronisation of the engine stream; each is bit-identical to `eos_prob` on that row.  `eos_logits` keeps the logits."""
+        h = self.hidden if hidden is None else hidden
+        self._row_of(h, "hidden")
+        r = N.i32(rows)
+        if h.dim() != 2 or not h.is_contiguous():
+            raise ValueError("hidden must be a contiguous [R, H]")
+        if not 1 <= len(r) <= self.EOS_MAX_ROWS or any(not 0 <= int(x) < h.shape[0] for x in r):
+            raise ValueError("rows %s: 1..%d rows of hidden's %d" % (list(rows), self.EOS_MAX_ROWS, h.shape[0]))
+        N.check(self.lib.vv_eos_prob_rows(self.h, C.c_void_p(h.data_ptr()), N.iptr(r), len(r), C.c_void_p(self.eos_d[0].data_ptr()),
+                                          C.c_void_p(self.eos_d[1].data_ptr()), self.s), "vv_eos_prob_rows")
+        return self._eos_read(len(r))
 
     # ---- KV -----------------------------------------------------------------------------------------
     def kv_init(self, total_tokens: int):

@@ -16,6 +16,9 @@ count of the requests in the queue per frame.
 Results do not depend on batch-mates: a request's output equals `torch.manual_seed(seed); model.generate(<that request alone>, ...)` with
 `set_ddpm_inference_steps(steps)` and that solver.  Each request has its own CPU generator (diffusion noise, `randn(2, 64)[:1]` per
 diffusion frame) and device generator (voice-prompt noise, then SDE step noise), drawn in the solo run's order.
+
+`StreamingRequestQueue` does the same for the streaming-0.5B variant (`streaming.py`), with per-request audio streamers and text that
+arrives while the request speaks (`push_text`).
 """
 from __future__ import annotations
 
@@ -347,3 +350,375 @@ class RequestQueue:
         self._pages_used -= row.req.pages
         return VibeVoiceGenerationOutput(sequences=torch.tensor([row.seq], dtype=torch.long), speech_outputs=[audio],
                                          reach_max_step_sample=torch.tensor([row.reach_max]))
+
+
+# ---- streaming-0.5B -------------------------------------------------------------------------------------------------------------------
+@dataclass
+class _StreamRequest:
+    rid: int
+    prompt: List[int]                   # input_ids when there is no cached prompt: run one token per tick after the negative token
+    prefilled: Any                      # all_prefilled_outputs, or None
+    neg_id: int
+    seq0: List[int]                     # the TTS-LM's view of the prompt: where `sequences` start
+    text: List[int]                     # every text token pushed so far
+    complete: bool
+    cfg_scale: float
+    steps: int
+    seed: int
+    max_length: int
+    pages: int                          # worst-case KV pages of the three sequences
+    streamer: Any
+
+
+@dataclass
+class _Slot:
+    req: _StreamRequest
+    gen: torch.Generator                # the request's `randn(2, vae)[:1]` frame noise
+    seq: List[int]
+    prompt: List[int]                   # prompt tokens still to run; the first one goes to the negative row while `neg_first`
+    neg_first: bool
+    window: List[int] = field(default_factory=list)     # text tokens of the current window still to run
+    taken: int = 0                      # text tokens taken into windows so far
+    frames: int = 0                     # speech frames left in the current window
+    audio: List[torch.Tensor] = field(default_factory=list)
+
+
+class StreamingRequestQueue:
+    """Continuous batching of streaming-0.5B requests over a `max_slots` model (`streaming.VibeVoiceStreamingForConditionalGenerationInference`).
+
+        q = StreamingRequestQueue(model, max_total_tokens=...)
+        rid = q.submit(**inputs, tts_text_ids=first_ids, text_complete=False, cfg_scale=1.5, steps=5, max_new_tokens=600, seed=0,
+                       audio_streamer=AudioStreamer(1))
+        q.push_text(rid, more_ids, complete=True)       # text may arrive while the request speaks
+        done = q.step()                                 # one tick; [(rid, VibeVoiceGenerationOutput)] of the requests that finished
+        for rid, out in q.run(): ...                    # or: tick until every request has finished
+
+    Every tick advances each slot by one unit of the solo loop (`streaming.generate`): one prompt token, one text token, or one speech
+    frame.  The slots' units share the launches: one lower-stack program for the slots on a text token, one sampler -> acoustic decoder ->
+    connector pass for the slots on a speech frame, one type-embedding launch, one upper-stack (TTS-LM) program for all of them (text
+    slots on one row, speech slots on both), and one EOS-classifier launch whose read-back is the tick's only host synchronisation.  A
+    slot takes its next text window when 5 tokens are pending, or fewer once its text is complete; until then it waits and takes part in
+    no launch, so the output does not depend on how the text was split into `push_text` calls.
+
+    A request's output equals `torch.manual_seed(seed); model.set_ddpm_inference_steps(steps); model.generate(<that request with its
+    whole text>, cfg_scale=cfg_scale)`: each request has its own CPU generator for the frame noise and its own sampler settings
+    (`Engine.set_row_sampler`).  At the EOS decision the slot is freed at once; the solo loop still runs the rest of that speech window,
+    whose audio it does not keep, so only its `1` tokens are appended to `sequences` here.  Audio reaches each request's streamer through
+    the engine's pinned ring after the tick's read-back.  Driven from one thread; streamers may be read from others."""
+
+    def __init__(self, model, max_total_tokens: int):
+        eng = model.engine
+        if eng is None or not eng.finalized:
+            raise N.VVError("weights not loaded")
+        self.model, self.eng, self.S = model, eng, model.max_slots
+        eng.kv_init(int(max_total_tokens))
+        self._budget = eng.kv_pages - 2 * eng.B            # every decode keeps one page for each sequence's next entry
+        self._waiting: Deque[_StreamRequest] = collections.deque()
+        self._reqs = {}                                    # rid -> request, until it has finished
+        self._slots: List[Optional[_Slot]] = [None] * self.S
+        self._next_rid = 0
+        self._pages_used = 0
+        self._nmax = 0
+        self._started = False
+        self._pending_audio: List[Tuple[Any, List[int], List[Any]]] = []
+        self.last_tick = (0, 0)                            # (slots on a text or prompt token, slots on a speech frame) of the last tick
+
+    # ---- requests ---------------------------------------------------------------------------------------------------------------------
+    def submit(self, inputs=None, tts_text_ids=None, text_complete: bool = True, cfg_scale: float = 1.0, steps: Optional[int] = None,
+               max_new_tokens: Optional[int] = None, seed: int = 0, audio_streamer=None, solver: str = "dpmsolver++",
+               stop_check_fn=None, **kwargs) -> int:
+        """Queue one request; takes what `generate()` takes (the processor's output, with or without `all_prefilled_outputs`).  Returns
+        the request id that `step()` / `run()` report."""
+        model = self.model
+        if stop_check_fn is not None:
+            raise ValueError("stop_check_fn is not supported by StreamingRequestQueue (use cancel(rid))")
+        if solver != "dpmsolver++":
+            raise ValueError("solver %r: the streaming loop samples with dpmsolver++ only" % (solver,))
+        steps = int(model.ddpm_inference_steps if steps is None else steps)
+        if not 1 <= steps <= model._max_steps:
+            raise ValueError("steps %d outside [1, %d] (the model's max_diffusion_steps)" % (steps, model._max_steps))
+        if audio_streamer is not None and getattr(audio_streamer, "batch_size", 1) != 1:
+            raise ValueError("audio_streamer must have batch size 1 (one streamer per request)")
+        tokenizer = kwargs.pop("tokenizer", None)
+        neg_id = kwargs.pop("neg_text_input_id", None)
+        prefilled = kwargs.pop("all_prefilled_outputs", None)
+        ids = kwargs["input_ids"] if "input_ids" in kwargs else inputs
+        if ids is None:
+            raise ValueError("input_ids are required")
+        ids = torch.as_tensor(ids).cpu().long()
+        if ids.dim() == 2:
+            if ids.shape[0] != 1:
+                raise ValueError("one request per submit (input_ids has %d rows)" % ids.shape[0])
+            ids = ids[0]
+        tts_ids = kwargs.get("tts_lm_input_ids")
+        tts_ids = ids if tts_ids is None else torch.as_tensor(tts_ids).cpu().long()
+        if tts_ids.dim() == 2 and tts_ids.shape[0] != 1:
+            raise ValueError("one request per submit (tts_lm_input_ids has %d rows)" % tts_ids.shape[0])
+        tts_ids = tts_ids.reshape(-1)
+        if prefilled is None and neg_id is None and tokenizer is None:
+            raise ValueError("without all_prefilled_outputs the negative prompt needs neg_text_input_id= or tokenizer=")
+        neg_id = 0 if prefilled is not None and neg_id is None and tokenizer is None else \
+            int(tokenizer.convert_tokens_to_ids("<|image_pad|>") if neg_id is None else neg_id)
+        text = [] if tts_text_ids is None else torch.as_tensor(tts_text_ids).cpu().long().reshape(-1).tolist()
+        L0 = int(tts_ids.numel())
+        mnt = model.config.decoder_config.max_position_embeddings - L0 if max_new_tokens is None else int(max_new_tokens)
+        if prefilled is not None:
+            lens = [self._cache_len(prefilled[k].past_key_values) for k in ("lm", "tts_lm", "neg_tts_lm")]
+        else:
+            lens = [int(ids.numel()), int(ids.numel()), 1]
+        pages = sum((n + mnt + 2 + 63) // 64 for n in lens)
+        if pages > self._budget:
+            raise ValueError("max_total_tokens: the request needs up to %d KV pages, the pool has %d for requests" % (pages, self._budget))
+        rid = self._next_rid
+        self._next_rid += 1
+        req = _StreamRequest(rid, [] if prefilled is not None else ids.tolist(), prefilled, neg_id, tts_ids.tolist(), text, bool(text_complete),
+                             float(cfg_scale), steps, int(seed), L0 + mnt, pages, audio_streamer)
+        self._waiting.append(req)
+        self._reqs[rid] = req
+        return rid
+
+    @staticmethod
+    def _cache_len(cache) -> int:
+        if hasattr(cache, "key_cache"):
+            return int(cache.key_cache[0].shape[2])
+        if hasattr(cache, "layers"):
+            return int(next(l.keys for l in cache.layers if getattr(l, "keys", None) is not None).shape[2])
+        return int(cache[0][0].shape[2])
+
+    def push_text(self, rid: int, ids, complete: bool = False):
+        """Append text token ids to request `rid` (while it waits or speaks); `complete=True` marks its text as whole."""
+        req = self._reqs.get(rid)
+        if req is None:
+            raise KeyError("request %r is not queued or live" % (rid,))
+        if req.complete:
+            raise ValueError("request %d: its text is already complete" % rid)
+        req.text += torch.as_tensor(ids).cpu().long().reshape(-1).tolist()
+        req.complete = bool(complete)
+
+    def cancel(self, rid: int) -> VibeVoiceGenerationOutput:
+        """End request `rid` now (between ticks): returns what it produced so far and ends its streamer."""
+        req = self._reqs.get(rid)
+        if req is None:
+            raise KeyError("request %r is not queued or live" % (rid,))
+        for s, slot in enumerate(self._slots):
+            if slot is not None and slot.req is req:
+                return self._finish(s, False)
+        self._waiting.remove(req)
+        del self._reqs[rid]
+        if req.streamer is not None:
+            req.streamer.end()
+        return VibeVoiceGenerationOutput(sequences=torch.tensor([req.seq0], dtype=torch.long), speech_outputs=[None],
+                                         reach_max_step_sample=torch.tensor([False]))
+
+    # ---- the loop ---------------------------------------------------------------------------------------------------------------------
+    def run(self) -> Iterator[Tuple[int, VibeVoiceGenerationOutput]]:
+        """Tick until nothing is queued or live; yields (request id, output) in completion order.  Raises RuntimeError when every live
+        request waits for text that is not complete (push_text from inside the loop, or use step())."""
+        while self._waiting or any(s is not None for s in self._slots):
+            done = self.step()
+            if not done and self.last_tick == (0, 0):
+                raise RuntimeError("every live request waits for text that is not complete (push_text(..., complete=True))")
+            for item in done:
+                yield item
+
+    def _start(self):
+        eng = self.eng
+        eng.codec_state_reset()
+        for s in range(2 * eng.B):
+            eng.kv_set_len(s, 0)
+        with torch.cuda.stream(eng.stream):
+            eng.feat.zero_()                               # no semantic branch: the connector adds RMSNorm(0) = 0
+            self._hsave = torch.empty_like(eng.hidden)
+        self._set_nmax(max([r.steps for r in self._waiting], default=1))
+        self._started = True
+
+    def _stop(self):
+        eng = self.eng
+        eng.set_row_mode([1] * (2 * eng.B))
+        eng.sampler_per_row(0)
+        eng.sync()
+        self._started = False
+
+    def _set_nmax(self, n: int):
+        """Per-row sampler with n steps per frame; re-sets the live slots' settings (switching clears them)."""
+        self._nmax = n
+        self.eng.sampler_per_row(n)
+        for s, slot in enumerate(self._slots):
+            if slot is not None:
+                self.eng.set_row_sampler(s, slot.req.steps, "dpmsolver++", slot.req.cfg_scale)
+
+    def _admit(self):
+        eng, model = self.eng, self.model
+        while self._waiting:
+            req = self._waiting[0]
+            free = [s for s in range(self.S) if self._slots[s] is None]
+            if not free or self._pages_used + req.pages > self._budget:
+                break
+            self._waiting.popleft()
+            self._pages_used += req.pages
+            s = free[0]
+            if req.steps > self._nmax:
+                self._set_nmax(req.steps)
+            eng.set_row_sampler(s, req.steps, "dpmsolver++", req.cfg_scale)
+            eng.codec_state_zero([s])
+            slot = _Slot(req, torch.Generator().manual_seed(req.seed), list(req.seq0), list(req.prompt), req.prefilled is None)
+            if req.prefilled is not None:
+                model._import_prefilled(req.prefilled, s)
+            self._slots[s] = slot
+
+    def _unit(self, slot: _Slot):
+        """The slot's unit of this tick: ("text", token, to_negative_row), ("speech",), ("wait",) or ("max",) (the window exceeds
+        max_length: the request ends)."""
+        if slot.neg_first:
+            return ("text", slot.req.neg_id, True)
+        if slot.prompt:
+            return ("text", slot.prompt[0], False)
+        if slot.window:
+            return ("text", slot.window[0], False)
+        if slot.frames:
+            return ("speech",)
+        req = slot.req
+        pending = len(req.text) - slot.taken
+        if pending < 5 and not req.complete:                                   # TTS_TEXT_WINDOW_SIZE
+            return ("wait",)
+        cur = req.text[slot.taken:slot.taken + 5]
+        slot.taken += len(cur)
+        slot.frames = 6                                                        # TTS_SPEECH_WINDOW_SIZE
+        if cur:
+            slot.seq += cur
+            if len(slot.seq) > req.max_length:
+                return ("max",)
+            slot.window = list(cur)
+            return ("text", cur[0], False)
+        return ("speech",)
+
+    def step(self) -> List[Tuple[int, VibeVoiceGenerationOutput]]:
+        """One tick (see the class docstring); returns [(request id, output)] of the requests that finished in it."""
+        eng, model, S = self.eng, self.model, self.S
+        if not self._started:
+            if not self._waiting:
+                self.last_tick = (0, 0)
+                return []
+            self._start()
+        self._admit()
+        done = []
+        text, speech = [], []                              # slots on a text token: (slot, token, upper row); slots on a speech frame
+        for s, slot in enumerate(self._slots):
+            if slot is None:
+                continue
+            u = self._unit(slot)
+            if u[0] == "max":
+                done.append((slot.req.rid, self._finish(s, True)))
+            elif u[0] == "text":
+                pos, _, neg = model.slot_rows(s)
+                text.append((s, u[1], neg if u[2] else pos))
+            elif u[0] == "speech":
+                speech.append(s)
+        self.last_tick = (len(text), len(speech))
+        src, typ, dst, up = [], [], [], []
+        if text:                                          # lower stack: the text slots' tokens, output into their `embeds` rows
+            toks = [0] * (2 * eng.B)
+            for s, t, _ in text:
+                toks[model.slot_rows(s)[1]] = int(t)
+            rows = [model.slot_rows(s)[1] for s, _, _ in text]
+            eng.embed_tokens(toks, eng.embeds)
+            eng.set_row_mode(model._mode(rows))
+            eng.lm_decode_range(0, model.low, False, out=eng.embeds)
+            eng.kv_commit(model._mode(rows))
+            for s, _, r in text:
+                src.append(model.slot_rows(s)[1])
+                typ.append(1)
+                dst.append(r)
+                up.append(r)
+        stepped = []                                       # speech slots that run the TTS-LM step (and the EOS classifier)
+        if speech:
+            vae = model.config.acoustic_vae_dim
+            noise = torch.cat([torch.randn(2, vae, generator=self._slots[s].gen)[:1] for s in speech])
+            eng.upload_frame_inputs(noise, speech)
+            eng.diffusion_sample(1.0)                      # per-row mode: steps and CFG scales are the slots' own
+            eng.codec_decode()
+            with torch.cuda.stream(eng.stream):
+                chunk = eng.audio[speech].clone()
+            streamers = [self._slots[s].req.streamer for s in speech]
+            if any(st is not None for st in streamers):
+                self._pending_audio.append((eng.stage_audio(speech), list(speech), streamers))
+            eng.connect()                                  # -> embeds[s] and embeds[B + s]
+            for i, s in enumerate(speech):
+                slot = self._slots[s]
+                slot.audio.append(chunk[i:i + 1])
+                slot.frames -= 1
+                slot.seq.append(1)
+                if len(slot.seq) > slot.req.max_length:
+                    continue
+                pos, _, neg = model.slot_rows(s)
+                src += [pos, pos]
+                typ += [0, 0]
+                dst += [pos, neg]
+                up += [pos, neg]
+                stepped.append(s)
+        if up:
+            eng.tts_type_embed_rows(eng.embeds, src, typ, dst, eng.embeds)
+            # the upper program writes every hidden row: keep the TTS-LM state of the live rows it does not run
+            keep = [r for s, slot in enumerate(self._slots) if slot is not None for r in model.slot_rows(s)[::2] if r not in up]
+            with torch.cuda.stream(eng.stream):
+                for r in keep:
+                    self._hsave[r].copy_(eng.hidden[r])
+            eng.set_row_mode(model._mode(up))
+            eng.lm_decode_range(model.low, model.low + model.tts_layers, True)
+            eng.kv_commit(model._mode(up))
+            with torch.cuda.stream(eng.stream):
+                for r in keep:
+                    eng.hidden[r].copy_(self._hsave[r])
+        for s, _, _ in text:
+            slot = self._slots[s]
+            if slot.neg_first:
+                slot.neg_first = False
+                eng.kv_set_len(model.slot_rows(s)[1], 0)       # the negative prompt's text stack is not used again
+            elif slot.prompt:
+                slot.prompt.pop(0)
+            else:
+                slot.window.pop(0)
+        probs = eng.eos_probs([model.slot_rows(s)[0] for s in stepped]) if stepped else []
+        self._deliver_audio()
+        for s in speech:
+            slot = self._slots[s]
+            if s in stepped:
+                if probs[stepped.index(s)] <= 0.5:
+                    continue
+                for _ in range(slot.frames):               # the rest of the solo loop's window: frames whose audio is not kept
+                    slot.seq.append(1)
+                    if len(slot.seq) > slot.req.max_length:
+                        break
+                done.append((slot.req.rid, self._finish(s, False)))
+            else:
+                done.append((slot.req.rid, self._finish(s, True)))
+        if not self._waiting and all(slot is None for slot in self._slots):
+            self._stop()
+        return done
+
+    def _deliver_audio(self):
+        """Hand the staged frames to their streamers (valid after the tick's read-back; otherwise fetch_audio waits for that frame)."""
+        for ticket, rows, streamers in self._pending_audio:
+            a = self.eng.fetch_audio(ticket)
+            for i, st in enumerate(streamers):
+                if st is not None:
+                    st.put(a[i:i + 1].unsqueeze(1), torch.tensor([0]))
+        self._pending_audio = []
+
+    def _finish(self, s: int, reach_max: bool) -> VibeVoiceGenerationOutput:
+        eng, slot = self.eng, self._slots[s]
+        self._deliver_audio()
+        if slot.req.streamer is not None:
+            slot.req.streamer.end()
+        eng.sync()
+        with torch.cuda.stream(eng.stream):
+            audio = torch.cat(slot.audio, dim=-1) if slot.audio else None
+        eng.sync()
+        for r in self.model.slot_rows(s):
+            eng.kv_set_len(r, 0)
+        eng.codec_state_zero([s])
+        self._slots[s] = None
+        self._pages_used -= slot.req.pages
+        del self._reqs[slot.req.rid]
+        return VibeVoiceGenerationOutput(sequences=torch.tensor([slot.seq], dtype=torch.long), speech_outputs=[audio],
+                                         reach_max_step_sample=torch.tensor([reach_max]))

@@ -6,13 +6,16 @@ What differs from the multi-speaker loop (`modeling.py`), and how it maps onto t
     LM" with the final norm.  Both live in the engine's one layer array (lower first); `vv_lm_decode_range` runs one stack at a time.
     Each stack has its own KV sequences because their lengths differ (the upper stack also sees the speech positions):
         row 0 = TTS-LM positive stream, row 1 = lower text stack, row 2 = TTS-LM negative stream (max_batch = 2, row 3 unused);
+    with `max_slots` = S > 1 the engine has max_batch = 2S and slot s uses rows s, S + s and 2S + s (`slot_rows`): the TTS-LM rows are
+    the sampler's positive / negative pair (rows b and B + b), and the lower stack takes positive rows the sampler never activates;
   * every TTS-LM input gets a type embedding added (1 = text, 0 = speech; `:290-291`): `vv_tts_type_embed`;
   * no token selection: windows of 5 text tokens alternate with 6 speech frames (`:40-42, :568-614`); a binary classifier on the TTS-LM
     hidden state ends the utterance (`:691-696`): `vv_eos_prob`, whose result is the one host sync per speech frame;
   * no semantic tokenizer: the frame is sampler -> acoustic decoder -> acoustic connector (`:617-645`).  The engine is given zero
     semantic weights, for which its connector stage returns exactly `acoustic_connector(latent)` (RMSNorm(0) = 0), and the semantic
     encoder stage is simply never launched.
-Batch size 1, like the reference (`:511`).
+Batch size 1 per `generate()`, like the reference (`:511`); a multi-slot model runs it in slot 0, and `serving.StreamingRequestQueue`
+serves up to `max_slots` requests at once.
 
 The native `Engine` always runs the type embeddings and the EOS classifier on its sm_90a kernels (`vv_tts_type_embed`, `vv_eos_prob`),
 and a checkpoint without their weights is refused.  An engine object that does not implement them (no `has_tts_heads`: the CPU
@@ -61,7 +64,12 @@ def remap_streaming_state_dict(items: Iterable[Tuple[str, torch.Tensor]], config
 
 
 class VibeVoiceStreamingForConditionalGenerationInference:
-    def __init__(self, config: VibeVoiceConfig, tts_backbone_num_hidden_layers: int = 20, device: int = 0, max_diffusion_steps: int = 64):
+    def __init__(self, config: VibeVoiceConfig, tts_backbone_num_hidden_layers: int = 20, device: int = 0, max_diffusion_steps: int = 64,
+                 max_slots: int = 1):
+        """`max_slots` (1..4): requests the engine can hold at once (`serving.StreamingRequestQueue`); the engine has 2 * max_slots rows."""
+        if not 1 <= int(max_slots) <= 4:
+            raise ValueError("max_slots must be in [1, 4] (max_batch = 2 * max_slots <= 8), got %r" % (max_slots,))
+        self.max_slots = int(max_slots)
         self.config = config
         self.tts_layers = int(tts_backbone_num_hidden_layers)
         self.low = config.decoder_config.num_hidden_layers - self.tts_layers
@@ -91,7 +99,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
         elif device_map is not None and device_map not in ("cuda", "auto"):
             raise N.VVError("vibevoice_b200 runs on CUDA devices only (device_map=%r); there is no CPU path" % (device_map,))
         m = cls(cfg, tts_backbone_num_hidden_layers=int(getattr(cfg, "tts_backbone_num_hidden_layers", 20)), device=dev,
-                max_diffusion_steps=int(kw.pop("max_diffusion_steps", 64)))
+                max_diffusion_steps=int(kw.pop("max_diffusion_steps", 64)), max_slots=int(kw.pop("max_slots", 1)))
         files = sorted(glob.glob(os.path.join(path, "*.safetensors")))
         if not files:
             raise FileNotFoundError("no *.safetensors under %s" % path)
@@ -118,7 +126,16 @@ class VibeVoiceStreamingForConditionalGenerationInference:
             _attn_implementation=getattr(self, "_attn_implementation", "paged-split-kv"))))
 
     def _new_engine(self):
-        return Engine(self.config, [0, 1], 2, self._device_index, self._max_steps)      # no token constraint here; ids are unused
+        return Engine(self.config, [0, 1], 2 * self.max_slots, self._device_index, self._max_steps)   # no token constraint; ids are unused
+
+    def slot_rows(self, slot: int) -> Tuple[int, int, int]:
+        """(TTS-LM positive, lower text stack, TTS-LM negative) rows of `slot`; slot 0 of a one-slot model is (ROW_POS, ROW_TEXT, ROW_NEG)."""
+        S = self.max_slots
+        return slot, S + slot, 2 * S + slot
+
+    def _mode(self, rows) -> List[int]:
+        """row modes of `vv_set_row_mode` with exactly `rows` on"""
+        return [1 if r in rows else 0 for r in range(4 * self.max_slots)]
 
     def load_state_dict(self, state_dict):
         eng = self.engine = self._new_engine()
@@ -156,24 +173,28 @@ class VibeVoiceStreamingForConditionalGenerationInference:
     def _lower_then_upper_text(self, token_ids: List[int], neg: bool = False):
         """One text token at a time: lower stack (row 1) -> upper stack (+ type 1) on the positive (or negative) TTS-LM row (:590-611)."""
         eng = self.engine
-        up_row = ROW_NEG if neg else ROW_POS
+        pos, text, negr = self.slot_rows(0)
+        up_row = negr if neg else pos
         for t in token_ids:
-            eng.embed_tokens([0, int(t), 0, 0], eng.embeds)
-            eng.set_row_mode([0, 1, 0, 0])
+            toks = [0] * (4 * self.max_slots)
+            toks[text] = int(t)
+            eng.embed_tokens(toks, eng.embeds)
+            eng.set_row_mode(self._mode([text]))
             eng.lm_decode_range(0, self.low, False)
-            eng.kv_commit([0, 1, 0, 0])
-            self._type_embed(eng.hidden[ROW_TEXT], 1, [up_row])
-            eng.set_row_mode([1 if r == up_row else 0 for r in range(4)])
+            eng.kv_commit(self._mode([text]))
+            self._type_embed(eng.hidden[text], 1, [up_row])
+            eng.set_row_mode(self._mode([up_row]))
             eng.lm_decode_range(self.low, self.low + self.tts_layers, True)
-            eng.kv_commit([1 if r == up_row else 0 for r in range(4)])
+            eng.kv_commit(self._mode([up_row]))
 
     def _speech_step(self, embed: torch.Tensor):
         """One TTS-LM step on both streams with the acoustic embedding (+ type 0) (:657-689)."""
         eng = self.engine
-        self._type_embed(embed, 0, [ROW_POS, ROW_NEG])
-        eng.set_row_mode([1, 0, 1, 0])
+        pos, _, neg = self.slot_rows(0)
+        self._type_embed(embed, 0, [pos, neg])
+        eng.set_row_mode(self._mode([pos, neg]))
         eng.lm_decode_range(self.low, self.low + self.tts_layers, True)
-        eng.kv_commit([1, 0, 1, 0])
+        eng.kv_commit(self._mode([pos, neg]))
 
     def _type_embed(self, src: torch.Tensor, type_id: int, rows: List[int]):
         """`embeds[r] = src + tts_input_types[type_id]` for r in rows (:290-291); src may be one of those rows."""
@@ -201,15 +222,16 @@ class VibeVoiceStreamingForConditionalGenerationInference:
     def _prefill_from_ids(self, input_ids: torch.Tensor, neg_id: int):
         """No cached prompt given: compute the four streams' prompt state through the decode kernels."""
         eng = self.engine
+        _, text, neg = self.slot_rows(0)
         self._lower_then_upper_text([neg_id], neg=True)
-        eng.kv_set_len(ROW_TEXT, 0)                            # the negative text stack is not used again (:527-534 only keep its kwargs)
+        eng.kv_set_len(text, 0)                                # the negative text stack is not used again (:527-534 only keep its kwargs)
         with torch.cuda.stream(eng.stream):
-            neg_hidden = eng.hidden[ROW_NEG].clone()
+            neg_hidden = eng.hidden[neg].clone()
         self._lower_then_upper_text(input_ids.tolist())
         with torch.cuda.stream(eng.stream):
-            eng.hidden[ROW_NEG].copy_(neg_hidden)               # conditions of the first frame: last prompt position of both TTS-LM streams
+            eng.hidden[neg].copy_(neg_hidden)                   # conditions of the first frame: last prompt position of both TTS-LM streams
 
-    def _import_prefilled(self, outs):
+    def _import_prefilled(self, outs, slot: int = 0):
         """`all_prefilled_outputs` (:517-534; the cached voice prompts of demo/streaming_inference_from_file.py:291 carry these four
         outputs): dict lm / tts_lm / neg_lm / neg_tts_lm of model outputs whose `past_key_values` expose per-layer key/value tensors
         [1, kv_heads, L, head_dim] (rotated keys, as HF caches them) and whose `last_hidden_state` is [1, L, H].  K/V go to the paged
@@ -234,12 +256,13 @@ class VibeVoiceStreamingForConditionalGenerationInference:
                 eng.kv_write(seq, layer0 + j, 0, k, v)
             eng.kv_set_len(seq, L)
             return L
-        put(outs["lm"].past_key_values, ROW_TEXT, 0, self.low)
-        put(outs["tts_lm"].past_key_values, ROW_POS, self.low, self.tts_layers)
-        put(outs["neg_tts_lm"].past_key_values, ROW_NEG, self.low, self.tts_layers)
+        pos, text, neg = self.slot_rows(slot)
+        put(outs["lm"].past_key_values, text, 0, self.low)
+        put(outs["tts_lm"].past_key_values, pos, self.low, self.tts_layers)
+        put(outs["neg_tts_lm"].past_key_values, neg, self.low, self.tts_layers)
         with torch.cuda.stream(eng.stream):
-            eng.hidden[ROW_POS].copy_(outs["tts_lm"].last_hidden_state[0, -1].to(eng.device, torch.float32))
-            eng.hidden[ROW_NEG].copy_(outs["neg_tts_lm"].last_hidden_state[0, -1].to(eng.device, torch.float32))
+            eng.hidden[pos].copy_(outs["tts_lm"].last_hidden_state[0, -1].to(eng.device, torch.float32))
+            eng.hidden[neg].copy_(outs["neg_tts_lm"].last_hidden_state[0, -1].to(eng.device, torch.float32))
 
     @torch.no_grad()
     def generate(self, inputs=None, tts_text_ids=None, cfg_scale: float = 1.0, audio_streamer=None, return_speech: bool = True,
@@ -269,7 +292,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
             eng.kv_init(4 * (max_length + 8))
         eng.set_diffusion_steps(int(self.ddpm_inference_steps))
         eng.codec_state_reset()
-        for s in range(4):
+        for s in range(4 * self.max_slots):
             eng.kv_set_len(s, 0)
         # ---- prefill: what `all_prefilled_outputs` carries (lm / tts_lm and their negatives) ----
         prefilled = kwargs.pop("all_prefilled_outputs", None)
@@ -278,6 +301,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
         else:
             self._prefill_from_ids(input_ids, neg_id)
 
+        neg_row = self.slot_rows(0)[2]
         seq: List[int] = tts_ids.tolist()
         chunks: List[torch.Tensor] = []
         finished, reach_max, win = False, False, 0
@@ -297,14 +321,14 @@ class VibeVoiceStreamingForConditionalGenerationInference:
                     reach_max = True
                     break
                 with torch.cuda.stream(eng.stream):
-                    neg_hidden = eng.hidden[ROW_NEG].clone()
+                    neg_hidden = eng.hidden[neg_row].clone()
                 self._lower_then_upper_text(cur.tolist())                                          # :590-611
                 with torch.cuda.stream(eng.stream):
-                    eng.hidden[ROW_NEG].copy_(neg_hidden)       # the text window does not touch the negative stream
+                    eng.hidden[neg_row].copy_(neg_hidden)       # the text window does not touch the negative stream
             for _ in range(TTS_SPEECH_WINDOW_SIZE):                                                # :614
                 noise = torch.randn(2, vae)[:1]                                                    # :741, CPU global generator
                 eng.upload_frame_inputs(noise, [0])
-                eng.diffusion_sample(cfg_scale)                                                    # :617-621 (rows 0 and B+0 = 2)
+                eng.diffusion_sample(cfg_scale)                                                    # :617-621 (rows 0 and B + 0)
                 eng.codec_decode()                                                                 # :624-632
                 with torch.cuda.stream(eng.stream):
                     chunk = eng.audio[0:1].clone()
@@ -315,7 +339,7 @@ class VibeVoiceStreamingForConditionalGenerationInference:
                     audio_streamer.put(chunk.unsqueeze(1), torch.tensor([0]))
                 with torch.cuda.stream(eng.stream):
                     eng.feat.zero_()
-                eng.connect()                                                                      # :645 -> eng.embeds[0] (and [2])
+                eng.connect()                                                                      # :645 -> eng.embeds[0] (and [B])
                 seq.append(1)                                                                      # :646
                 if len(seq) > max_length:                                                          # :648-649
                     break
