@@ -67,7 +67,8 @@ typedef struct {
   int32_t n_valid_ids;
   int32_t valid_ids[8];
   /* runtime sizing */
-  int32_t max_batch;                /* B: samples resident on this GPU */
+  int32_t max_batch;                /* B: samples resident on this GPU, 1..16 (2B <= 32 sequences: the largest MMA operand of the
+                                       weight-stream kernel); vv_create refuses anything else */
   int32_t max_diffusion_steps;      /* upper bound for vv_set_diffusion_steps */
 } vv_model_desc;
 
@@ -198,7 +199,7 @@ int vv_voice_encode(vv_ctx* ctx, const float* wavs /*[n,T] fp32*/, int n, int64_
 int64_t vv_lm_prefill_workspace(vv_ctx* ctx, int64_t n_tokens);          /* minimum workspace bytes of the call below */
 int vv_lm_prefill(vv_ctx* ctx, int seq, int64_t pos0, int64_t n_tokens, const float* embeds, float* hidden_last, void* workspace,
                   int64_t workspace_bytes, void* stream);
-/* embedding rows of DEVICE token ids (any count; vv_embed_tokens takes at most 16 host ids): out [n,H] fp32; ids outside [0, vocab) give
+/* embedding rows of DEVICE token ids (any count; vv_embed_tokens takes at most 32 host ids): out [n,H] fp32; ids outside [0, vocab) give
  * zero rows. */
 int vv_embed_gather(vv_ctx* ctx, const int32_t* ids_dev, int64_t n, float* out, void* stream);
 

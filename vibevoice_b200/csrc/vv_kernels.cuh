@@ -818,6 +818,8 @@ __global__ void advance_kernel(const StateSeg* __restrict__ segs, const int* __r
 // ---------------------------------------------------------------------------------------------
 // LLM decode step pieces
 // ---------------------------------------------------------------------------------------------
+constexpr int MAX_BATCH = 16;   // samples per GPU: 2B = 32 sequences = the weight-stream kernel's largest MMA operand (vv_stream.cuh, nB = 64)
+constexpr int MAX_SEQ = 2 * MAX_BATCH;
 constexpr int KV_PAGE = 64;     // tokens per page
 constexpr int HD = 128;         // head_dim of both shipped models (configs/*.json)
 

@@ -693,7 +693,8 @@ extern "C" const char* vv_last_error(void) { return g_err.c_str(); }
 extern "C" int vv_create(const vv_model_desc* desc, int device, vv_ctx** out) {
   if (!desc || !out) return fail(VV_ERR_INVALID, "vv_create: null argument");
   if (desc->head_dim != 128 && desc->head_dim != 64) return fail(VV_ERR_INVALID, "head_dim %d unsupported (64 or 128)", desc->head_dim);
-  if (desc->max_batch < 1 || desc->max_batch > 8) return fail(VV_ERR_INVALID, "max_batch must be in [1,8]");
+  if (desc->max_batch < 1 || desc->max_batch > MAX_BATCH)
+    return fail(VV_ERR_INVALID, "max_batch %d outside [1,%d] (2 * max_batch sequences, at most %d rows per MMA operand)", desc->max_batch, MAX_BATCH, MAX_SEQ);
   if (desc->n_stages < 2 || desc->n_stages > 8) return fail(VV_ERR_INVALID, "n_stages out of range");
   if (desc->num_q_heads % desc->num_kv_heads || desc->num_q_heads / desc->num_kv_heads > ATT_MAXG)
     return fail(VV_ERR_INVALID, "GQA group size unsupported");
@@ -1219,11 +1220,11 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
   RET(dmalloc(c, &c->s_pacc2, (size_t)M2 * d.num_kv_heads * c->sm_count * 8 * HD));
   RET(dmalloc(c, &c->s_pml2, (size_t)M2 * d.num_kv_heads * c->sm_count * 8 * 2));
   RET(dmalloc(c, &c->s_tok, 64));
-  RET(dmalloc(c, &c->kv_len_dev, 16));
-  RET(dmalloc(c, &c->row_mode_dev, 16));
+  RET(dmalloc(c, &c->kv_len_dev, MAX_SEQ));
+  RET(dmalloc(c, &c->row_mode_dev, MAX_SEQ));
   {
-    int ones[16];
-    for (int i = 0; i < 16; ++i) ones[i] = 1;
+    int ones[MAX_SEQ];
+    for (int i = 0; i < MAX_SEQ; ++i) ones[i] = 1;
     CK(cudaMemcpy(c->row_mode_dev, ones, sizeof ones, cudaMemcpyHostToDevice));
   }
   c->kv_len_host.assign(M2, 0);
@@ -1366,13 +1367,13 @@ static void release_pages(vv_ctx* c, int seq, int64_t len) {
   while (pg.size() > keep) { c->free_pages.push_back(pg.back()); pg.pop_back(); }
 }
 
-struct Lens { int v[16]; };
+struct Lens { int v[MAX_SEQ]; };
 __global__ void kv_set_all_kernel(int* kv_len, Lens l, int n) { if (threadIdx.x < n) kv_len[threadIdx.x] = l.v[threadIdx.x]; }
 
 static int push_lens(vv_ctx* c, cudaStream_t s) {
   Lens l;
   const int n = 2 * c->d.max_batch;
-  for (int i = 0; i < 16; ++i) l.v[i] = i < n ? (int)c->kv_len_host[i] : 0;
+  for (int i = 0; i < MAX_SEQ; ++i) l.v[i] = i < n ? (int)c->kv_len_host[i] : 0;
   kv_set_all_kernel<<<1, 32, 0, s>>>(c->kv_len_dev, l, n);
   CKL();
   c->launches++;
@@ -1425,7 +1426,7 @@ extern "C" int vv_kv_delete_slot(vv_ctx* c, int seq, int64_t pos, void* stream) 
 extern "C" int vv_set_row_mode(vv_ctx* c, const int32_t* rm, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
   Lens l;
-  for (int i = 0; i < 16; ++i) l.v[i] = i < 2 * c->d.max_batch ? rm[i] : 0;
+  for (int i = 0; i < MAX_SEQ; ++i) l.v[i] = i < 2 * c->d.max_batch ? rm[i] : 0;
   kv_set_all_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(c->row_mode_dev, l, 2 * c->d.max_batch);
   CKL();
   c->launches++;
@@ -1553,7 +1554,7 @@ extern "C" int vv_lm_logits_full(vv_ctx* c, const float* hidden, float* logits_o
   GemvP p = mk(c->lm_head_w, nullptr, hidden, c->d.hidden_size, logits_out, c->d.vocab_size, c->d.max_batch, c->d.vocab_size, c->d.hidden_size);
   return linear(l, p);
 }
-struct Toks { int v[16]; };
+struct Toks { int v[MAX_SEQ]; };
 __global__ void embed_gather_val_kernel(const bf16* __restrict__ table, Toks t, float* __restrict__ out, int H) {
   const bf16* row = table + (size_t)t.v[blockIdx.x] * H;
   for (int k = threadIdx.x; k < H; k += blockDim.x) out[(size_t)blockIdx.x * H + k] = __bfloat162float(row[k]);
@@ -1572,9 +1573,9 @@ extern "C" int vv_lm_decode_range(vv_ctx* c, const float* embeds, int layer_begi
 
 extern "C" int vv_embed_tokens(vv_ctx* c, const int32_t* tokens_host, int n, float* out, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  if (n < 1 || n > 16) return fail(VV_ERR_INVALID, "vv_embed_tokens: n must be in [1,16]");
+  if (n < 1 || n > MAX_SEQ) return fail(VV_ERR_INVALID, "vv_embed_tokens: n must be in [1,%d]", MAX_SEQ);
   Toks t;
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < MAX_SEQ; ++i) {
     t.v[i] = i < n ? tokens_host[i] : 0;
     if (t.v[i] < 0 || t.v[i] >= c->d.vocab_size) return fail(VV_ERR_INVALID, "token id %d out of range", t.v[i]);
   }
@@ -2020,7 +2021,7 @@ static int conv_apply(const L& l, const ConvL& cv, const float* win, float* y, i
   return linear(l, p);
 }
 
-// ---- codec stages with B*T <= 8 rows (96 % of the codec's weights: 2048- and 1024-wide blocks, stem / up- / down-sampling convolutions
+// ---- codec stages with T <= 8 frames and B*T <= 32 rows (96 % of the codec's weights: 2048- and 1024-wide blocks, stem / up- / down-sampling convolutions
 // next to them) as weight-stream programs (vv_stream.cuh: SP_WINDOW, SP_MIXER): two stages per Block1D instead of five kernels ------------
 // Buffers: rows ping-pong between X[0] / X[1], FFN hidden sums between U[0] / U[1].  A block reads X[a], its owner CTA stores x1 into X[a^1]
 // and the second linear accumulates there; a convolution accumulates into a ZEROED buffer -- zero-fill jobs ride on the stage after the
@@ -2073,7 +2074,7 @@ static int stage_ops(StreamBuilder& b, vv_ctx* c, CodecBufs& cb, const std::vect
   return 0;
 }
 
-// decoder front: stem conv + the leading stages with <= 8 rows; *n_front = stages covered (at least stage 0: T = 1, B <= 8 rows), *out_x =
+// decoder front: stem conv + the leading stages codec_stream_stage accepts; *n_front = stages covered (at least stage 0: T = 1, B <= 16 rows), *out_x =
 // where the last one leaves its rows
 static int dec_front_stages(const vv_ctx* c) {
   int nf = 1;
@@ -2120,7 +2121,7 @@ static int dec_front_prog(vv_ctx* c, const float* latent, const vv_ctx::StreamPr
   return 0;
 }
 
-// encoder back: the trailing stages with <= 8 rows (at least the last one: T = 1, B <= 8 rows), each behind its strided conv, + the head
+// encoder back: the trailing stages codec_stream_stage accepts (at least the last one: T = 1, B <= 16 rows), each behind its strided conv, + the head
 // conv.  `xin` = rows entering the conv of the first covered stage (produced by the kernel-per-stage path).
 static int enc_back_first(const vv_ctx* c) {
   const Codec& k = c->enc;
@@ -2288,20 +2289,28 @@ static int enqueue_encode(const L& l, const float* audio, const int32_t* active,
   return 0;
 }
 
+// Both connectors in groups of at most CONNECT_ROWS rows: fc2's RMSNorm prologue at K = H > 512 runs only on the GEMV path (M <= 8), so
+// B > 8 reads the connector weights (~10 MB at 1.5B) once per group instead of needing a second kernel.  B <= 8 is one group.
+constexpr int CONNECT_ROWS = 8;
 static int enqueue_connect(const L& l, const float* latent, const float* sem, const int32_t* active, float* embeds) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
-  const int H = d.hidden_size, B = d.max_batch;
-  GemvP p = mk(c->ca_fc1, c->ca_b1, latent, 64, c->s_c1, H, B, H, 64);
-  RET(linear(l, p));
-  p = mk(c->ca_fc2, c->ca_b2, c->s_c1, H, c->s_e, H, B, H, H);
-  p.pro = PRO_RMSNORM; p.pro_w = c->ca_n; p.pro_eps = 1e-6f;
-  RET(linear(l, p));
-  p = mk(c->cs_fc1, c->cs_b1, sem, d.semantic_vae_dim, c->s_c1, H, B, H, d.semantic_vae_dim);
-  RET(linear(l, p));
-  p = mk(c->cs_fc2, c->cs_b2, c->s_c1, H, c->s_e, H, B, H, H);
-  p.pro = PRO_RMSNORM; p.pro_w = c->cs_n; p.pro_eps = 1e-6f; p.epi = EPI_RESID; p.res = c->s_e; p.ldres = H;
-  RET(linear(l, p));
+  const int H = d.hidden_size, B = d.max_batch, S = d.semantic_vae_dim;
+  for (int r0 = 0; r0 < B; r0 += CONNECT_ROWS) {
+    const int n = std::min(CONNECT_ROWS, B - r0);
+    float* c1 = c->s_c1 + (size_t)r0 * H;
+    float* e = c->s_e + (size_t)r0 * H;
+    GemvP p = mk(c->ca_fc1, c->ca_b1, latent + (size_t)r0 * 64, 64, c1, H, n, H, 64);
+    RET(linear(l, p));
+    p = mk(c->ca_fc2, c->ca_b2, c1, H, e, H, n, H, H);
+    p.pro = PRO_RMSNORM; p.pro_w = c->ca_n; p.pro_eps = 1e-6f;
+    RET(linear(l, p));
+    p = mk(c->cs_fc1, c->cs_b1, sem + (size_t)r0 * S, S, c1, H, n, H, S);
+    RET(linear(l, p));
+    p = mk(c->cs_fc2, c->cs_b2, c1, H, e, H, n, H, H);
+    p.pro = PRO_RMSNORM; p.pro_w = c->cs_n; p.pro_eps = 1e-6f; p.epi = EPI_RESID; p.res = e; p.ldres = H;
+    RET(linear(l, p));
+  }
   CK(launch_k(l, select_embeds_kernel, dim3(B), dim3(256), 0, embeds, c->s_e, active, B, H));
   return 0;
 }
@@ -2883,7 +2892,7 @@ extern "C" int vv_debug_kv_read(vv_ctx* c, int seq, int layer, int64_t pos0, int
   return 0;
 }
 
-struct Rows { int v[16]; };
+struct Rows { int v[MAX_BATCH]; };
 __global__ void state_zero_val_kernel(const StateSeg* __restrict__ segs, Rows r) {
   const int b = r.v[blockIdx.y];
   const StateSeg s = segs[blockIdx.x];
@@ -2895,7 +2904,7 @@ extern "C" int vv_codec_state_zero(vv_ctx* c, const int32_t* rows_host, int n, v
   if (n < 1) return 0;
   if (n > c->d.max_batch) return fail(VV_ERR_INVALID, "too many rows");
   Rows r;
-  for (int i = 0; i < 16; ++i) r.v[i] = i < n ? rows_host[i] : 0;
+  for (int i = 0; i < MAX_BATCH; ++i) r.v[i] = i < n ? rows_host[i] : 0;
   for (int i = 0; i < n; ++i) if (r.v[i] < 0 || r.v[i] >= c->d.max_batch) return fail(VV_ERR_INVALID, "row %d out of range", r.v[i]);
   cudaStream_t s = (cudaStream_t)stream;
   state_zero_val_kernel<<<dim3(c->dec.n_segs, n), 256, 0, s>>>(c->dec.segs_dev, r);
@@ -2907,7 +2916,7 @@ extern "C" int vv_codec_state_zero(vv_ctx* c, const int32_t* rows_host, int n, v
 }
 extern "C" int vv_codec_state_reset(vv_ctx* c, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  int rows[8];
+  int rows[MAX_BATCH];
   for (int i = 0; i < c->d.max_batch; ++i) rows[i] = i;
   return vv_codec_state_zero(c, rows, c->d.max_batch, stream);
 }

@@ -426,7 +426,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
   __shared__ unsigned long long full_bar[ST_MAX_STAGES], empty_bar[ST_MAX_STAGES];
   __shared__ float s_red[4][8];
   __shared__ float s_inv[64];
-  __shared__ float s_z[8 * 64];
+  // z' of every sample (SP_DPM); the 16-row-operand variants run B <= 4 samples and keep the smaller table
+  __shared__ float s_z[(((FEAT >> 29) & 1u) != 0u ? 8 : MAX_BATCH) * 64];
   __shared__ __align__(16) unsigned char s_opbuf[2][sizeof(SOp)];
   __shared__ int s_pinfo[128];
   const unsigned raw_addr = smem_u32(st_raw);
@@ -436,8 +437,11 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int NS = P.n_stages;
   const unsigned G = gridDim.x;
-  __shared__ int s_kvlen[16], s_rmode[16];
-  if (tid < 16) {
+  // sequence state: only programs with attention stages read it (the RoPE table is a job of the LM program's QKV stage).  The other
+  // families keep 16 entries, so their static shared memory -- which sets the ring depth of every codec and sampler program -- stays put.
+  constexpr int NSEQ = ((FEAT >> (16 + SK_ATTN)) & 1u) != 0u ? MAX_SEQ : 16;
+  __shared__ int s_kvlen[NSEQ], s_rmode[NSEQ];
+  if (tid < NSEQ) {
     s_kvlen[tid] = (P.kv_len && tid < P.n_seq) ? P.kv_len[tid] : 0;
     s_rmode[tid] = (P.row_mode && tid < P.n_seq) ? P.row_mode[tid] : 0;
   }
