@@ -132,14 +132,19 @@ int vv_embed_tokens(vv_ctx* ctx, const int32_t* tokens_host, int n, float* out /
 /* ---- a-4: CFG diffusion sampler (sample_speech_tokens :697-710 + dpm_solver.py) ---------------- */
 /* set_ddpm_inference_steps (:146) + scheduler.set_timesteps: the host computes the DPM-Solver++ scalar
  * tables (vibevoice_b200/schedule.py mirrors dpm_solver.py:321-423) and hands them over:
- * timesteps[n] (as float), coef[n][6] = {a0, s0, ks, kx, rinv, order}.  The sample-independent
- * timestep embeddings t_embedder(t_i) are computed here once. */
+ * timesteps[n] (as float), coef[n][6] = {a0, s0, ks, kx, rinv, order}.  Every row gets these settings (the sampler's per-row
+ * tables below, filled alike) and the CFG scale of the sampling call; the timestep embeddings t_embedder(t_i) are computed here once.
+ * Leaves per-row mode.  Captured sampler / frame-tail graphs are dropped only when n differs from the previous step count. */
 int vv_set_diffusion_steps(vv_ctx* ctx, int n_steps, const float* timesteps, const float* coef, void* stream);
 /* `algorithm_type='sde-dpmsolver++'` (the Gradio demo's scheduler, demo/gradio_demo.py:141-146; dpm_solver.py:680-686, 785-793):
  * coef7[n][7] = {a0, s0, ks, kx, rinv, order, kn}; the update adds kn * step_noise[step].  The reference draws that noise with
  * randn_tensor(model_output.shape) once per step on the model's device (dpm_solver.py:993-997); the caller provides the rows it
- * needs as step_noise [n_steps][B][64] fp32 (device, persistent) through vv_set_step_noise before vv_diffusion_sample/vv_frame_tail. */
+ * needs through vv_set_step_noise before vv_diffusion_sample/vv_frame_tail. */
 int vv_set_diffusion_steps_sde(vv_ctx* ctx, int n_steps, const float* timesteps, const float* coef7, void* stream);
+/* step_noise [n_max][B][64] fp32 (device, persistent; n_max = the step count of vv_set_diffusion_steps or vv_sampler_per_row): row r's
+ * noise of solver step j of the frame at step_noise[j][r].  Rows on dpmsolver++ add 0 times their entries,
+ * so those must be finite.  Binding another pointer drops the
+ * captured sampler / frame-tail graphs. */
 int vv_set_step_noise(vv_ctx* ctx, const float* step_noise);
 /* cond [2B,H] fp32 = LM hidden (rows as above); noise [B,64] fp32 = rows [0:n] of the reference's CPU
  * draw scattered to their sample slots; active[B] int32 (device) marks rows in diffusion mode.
@@ -149,13 +154,15 @@ int vv_diffusion_sample(vv_ctx* ctx, const float* cond, const float* noise, cons
 /* Per-row sampler settings (a request queue mixes step counts, solvers and CFG scales in one batch; demo/gradio_demo.py:141-147, 568
  * exposes all three per request).  vv_sampler_per_row(n_max > 0) switches the sampler to per-row mode: every row runs n_max solver steps
  * per frame, and each row starts as n_max identity steps on a zero timestep embedding with CFG scale 1 (its latent is its noise);
- * n_max = 0 switches back to the global mode of vv_set_diffusion_steps.  Switching drops the captured sampler / frame-tail graphs.
+ * n_max = 0 leaves the sampler unset (sampling fails with VV_ERR_STATE) until the next vv_set_diffusion_steps.  A change of the step
+ * count drops the captured sampler / frame-tail graphs.
  * vv_set_row_sampler sets row `row` (< B) to n_steps <= n_max steps: timesteps[n_steps] and coef[n_steps][ncol] as for
  * vv_set_diffusion_steps (ncol 6, dpmsolver++) or vv_set_diffusion_steps_sde (ncol 7, sde-dpmsolver++), and its CFG scale.  The row runs
  * n_max - n_steps identity steps conditioned on its first timestep, then its own steps, so its latent is that of a solo run with these
  * settings.  It writes device memory only: no program is rebuilt and no graph captured.  Step noise for row r's step j lives at
- * step_noise[n_max - n_steps + j][r] (vv_set_step_noise, [n_max][B][64]), needed once any row is on sde-dpmsolver++.  In per-row mode
- * vv_diffusion_sample and vv_frame_tail ignore their cfg_scale argument.  Synchronises the stream. */
+ * step_noise[n_max - n_steps + j][r] (vv_set_step_noise), needed once any row is on sde-dpmsolver++.  In per-row mode
+ * vv_diffusion_sample and vv_frame_tail ignore their cfg_scale argument.  vv_set_row_sampler outside per-row mode: VV_ERR_STATE.
+ * Synchronises the stream. */
 int vv_sampler_per_row(vv_ctx* ctx, int n_max, void* stream);
 int vv_set_row_sampler(vv_ctx* ctx, int row, int n_steps, const float* timesteps, const float* coef, int ncol /*6 ODE, 7 SDE*/,
                        float cfg_scale, void* stream);
@@ -263,8 +270,8 @@ int vv_debug_codec_taps(vv_ctx* ctx, int which, const float* in, const int32_t* 
  *   [2B][H], 5 head output v [2B][64], 6 z_{i+1} [B][64], 7 x0_i [B][64], 8 x = noisy_images_proj(z_{i+1}) [2B][H]; last, kind 9 latent_out.
  * kernel / split: kinds 0-3 = the {kernel, split-K factor} linear() ran (numbering as vv_debug_gemv2); block taps = the stream-kernel variant
  * and the number of stages (after the K split) of the block that wrote them.  taps == NULL: fills meta (kernel -1) and returns n_taps,
- * nothing launched.  Too little tap space: VV_ERR_INVALID with nothing launched; before vv_set_diffusion_steps (or SDE without step noise):
- * VV_ERR_STATE.  Returns n_taps.  Synchronises. */
+ * nothing launched.  Too little tap space: VV_ERR_INVALID with nothing launched; before vv_set_diffusion_steps, in per-row mode or on
+ * SDE without step noise: VV_ERR_STATE.  Returns n_taps.  Synchronises. */
 int vv_debug_sampler_taps(vv_ctx* ctx, const float* cond, const float* noise, float cfg_scale, float* latent_out, float* taps,
                           int64_t taps_floats, int32_t* meta, void* stream);
 /* Decoder layer `layer` of vv_lm_prefill alone, over n rows of sequence `seq` at positions [pos0, pos0 + n), from the fp32 residual input

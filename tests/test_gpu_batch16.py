@@ -72,8 +72,8 @@ def test_sampler_vs_oracle_b16(preset, B):
 
 @pytest.mark.parametrize("preset", ["1.5b-l2", "7b-l2"])
 def test_per_row_solver_b16(preset):
-    """16 rows of the per-row sampler with 5 / 10 / 20 steps, ODE and SDE mixed: each row against the same row sampled alone in the global
-    mode and against the oracle."""
+    """16 rows of the per-row sampler with 5 / 10 / 20 steps, ODE and SDE mixed: each row against the same row sampled alone with
+    `set_diffusion_steps` and against the oracle."""
     from oracle import vv_oracle as O
     from vibevoice_b200.schedule import DPMSolverMultistepScheduler
     B = 16

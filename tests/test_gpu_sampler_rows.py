@@ -1,7 +1,8 @@
 """The sampler's per-row mode (`vv_sampler_per_row` / `vv_set_row_sampler`): B = 4 rows with their own step counts, CFG scales and solvers
-in one program.  Each row's latent must match the same row sampled alone in the global mode with its own settings and the oracle sampler;
-rows on equal settings match the global mode; changing one row's settings leaves the others alone and builds no program; a non-finite
-row does not reach the others; a 1-step row among rows of max_diffusion_steps steps gives its 1-step result."""
+in one program.  Each row's latent must match the same row sampled alone with its own settings through `set_diffusion_steps` and the
+oracle sampler; rows on equal settings match the same settings given to every row by `set_diffusion_steps`; changing one row's settings
+leaves the others alone and builds no program; a non-finite row does not reach the others; a 1-step row among rows of
+max_diffusion_steps steps gives its 1-step result."""
 import os
 
 import pytest
@@ -55,7 +56,7 @@ def scheduler(eng, solver):
 
 
 def global_row(eng, cond, noise, step_noise, r, steps, cfg_scale, solver):
-    """Row r alone in the global mode (the other rows inactive)."""
+    """Row r alone with `set_diffusion_steps` (the other rows inactive)."""
     eng.sampler_per_row(0)
     eng.set_scheduler(scheduler(eng, solver))
     eng.set_diffusion_steps(steps)

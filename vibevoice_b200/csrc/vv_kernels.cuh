@@ -874,20 +874,7 @@ __global__ void __launch_bounds__(256) lm_head_argmax_kernel(const float* __rest
 // ---------------------------------------------------------------------------------------------
 // diffusion sampler glue
 // ---------------------------------------------------------------------------------------------
-// c_all[i][r][:] = silu(condp[r][:] + temb[i][:])   for all steps i (sample-independent t-embedding)
-__global__ void head_cond_prep_kernel(const float* __restrict__ condp, const float* __restrict__ temb, float* __restrict__ c_all,
-                                      int n_steps, int R, int H) {
-  pdl_trigger();
-  pdl_wait();
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long long)n_steps * R * H) return;
-  const int k = (int)(idx % H);
-  const int r = (int)((idx / H) % R);
-  const int i = (int)(idx / ((long long)H * R));
-  c_all[idx] = silu_f(condp[(size_t)r * H + k] + temb[(size_t)i * H + k]);
-}
-
-// per-row sampler: c_all[i][r][:] = silu(condp[r][:] + temb_rows[r mod B][i][:])   (each sample has its own timestep table)
+// c_all[i][r][:] = silu(condp[r][:] + temb_rows[r mod B][i][:])   for all steps i (each sample has its own timestep table)
 __global__ void head_cond_prep_rows_kernel(const float* __restrict__ condp, const float* __restrict__ temb_rows, float* __restrict__ c_all,
                                            int n_steps, int R, int B, int H) {
   pdl_trigger();

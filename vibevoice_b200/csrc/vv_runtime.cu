@@ -112,13 +112,15 @@ struct vv_ctx {
   // head
   bf16 *h_noisy = nullptr, *h_cond = nullptr, *h_t0 = nullptr, *h_t2 = nullptr, *h_mod = nullptr, *h_final = nullptr;
   std::vector<HeadLayer> head;
-  int n_steps = 0; float* temb = nullptr; float* tfreqs = nullptr;
+  float* tfreqs = nullptr;
   int32_t temb_info[2][2] = {{-1, 0}, {-1, 0}};   // {kernel, split-K} linear() ran for t_embedder.mlp.0 / .2 (vv_debug_sampler_taps)
-  std::vector<DpmCoef> coef_host; int coef_version = 0;
-  bool sde = false; const float* step_noise = nullptr;   // sde-dpmsolver++: per-step variance noise [n_steps][B][64] (vv_set_step_noise)
-  // per-row sampler (vv_sampler_per_row): row_nmax > 0 steps per frame for every row, settings in device tables written by vv_set_row_sampler
+  // sampler settings: row_nmax solver steps per frame for every row, each row's coefficients, CFG scale and timestep embeddings in device
+  // tables (vv_set_diffusion_steps writes every row alike, vv_set_row_sampler one row); row_nmax = 0: not set
   int row_nmax = 0; DpmCoef* row_coef = nullptr; float* row_cfg = nullptr; float* row_temb = nullptr;   // [nmax][B], [B], [B][nmax][H]
   std::vector<int> row_sde;              // rows whose settings add step noise
+  bool uniform = false;                  // every row has vv_set_diffusion_steps' settings and the sampling call's CFG scale
+  float cfg_last = NAN;                  // uniform: the CFG scale every row_cfg entry holds (NAN: not written yet)
+  const float* step_noise = nullptr;     // sde-dpmsolver++: per-step variance noise [row_nmax][B][64] (vv_set_step_noise)
   // connectors
   bf16 *ca_fc1 = nullptr, *ca_fc2 = nullptr, *cs_fc1 = nullptr, *cs_fc2 = nullptr;
   float *ca_b1 = nullptr, *ca_b2 = nullptr, *ca_n = nullptr, *cs_b1 = nullptr, *cs_b2 = nullptr, *cs_n = nullptr;
@@ -158,7 +160,6 @@ struct vv_ctx {
                                                                                          // per (weight, first column, columns)
   long long* st_trace2 = nullptr;
   long long* st_trace = nullptr; int st_trace_ops = 0; int st_trace_cta = 0; int st_trace_last_ops = 0;   // VV_STREAM_TRACE=<cta>: per-stage clock stamps of one CTA
-  float* cfg_dev = nullptr; float cfg_last = NAN;   // CFG scale lives in device memory so captured graphs do not depend on its value
   int64_t launches = 0;
   std::map<long long, int> occ_cache;
 };
@@ -359,7 +360,6 @@ struct StreamBuilder {
   std::vector<SOp> ops;
   std::vector<CUtensorMap> tmaps;
   std::vector<const bf16*> wsrc;   // op -> weight [N][K] of a linear stage (else null); sliced, packed and mapped by finish_stream
-  bool dpm_rows = false;           // the SP_DPM stages read per-row tables (runs on an SF_DPMROW variant)
   explicit StreamBuilder(vv_ctx* c_) : c(c_) {}
   SOp& push(int kind, bool sync) {
     SOp o;
@@ -448,18 +448,15 @@ constexpr unsigned SF_CODEC = sfeat({SP_NONE, SP_WINDOW, SP_RMSNORM, SP_GELU}, {
 constexpr unsigned SF_HD128 = 1u << 30;          // every attention stage has head_dim 128 (compile-time loop bounds)
 constexpr unsigned SF_LM128 = SF_LM | SF_HD128;
 constexpr unsigned SF_NB16 = 1u << 29;           // every linear stage has a 16-row activation operand (compile-time nB)
-constexpr unsigned SF_DPMROW = 1u << 28;         // the solver-update prologue reads per-row coefficients and CFG scales (vv_sampler_per_row)
-constexpr unsigned SF_ALL = 0xffffffffu & ~SF_HD128 & ~SF_NB16 & ~SF_DPMROW;
+constexpr unsigned SF_ALL = 0xffffffffu & ~SF_HD128 & ~SF_NB16;
 typedef void (*StreamFn)(SParams);
 static const struct { unsigned feat; StreamFn fn; StreamFn fn_trace; const char* name; } STREAM_VARIANTS[] = {
 #define SVAR(f, name) {f, stream_kernel<f, false>, stream_kernel<f, true>, name}
   SVAR(SF_SAMP | SF_NB16, "sampler (16-row operand)"), SVAR(SF_SAMP, "sampler"),
   SVAR(SF_LM128 | SF_NB16, "lm (head_dim 128, 16-row operand)"), SVAR(SF_LM128, "lm (head_dim 128)"), SVAR(SF_LM, "lm"),
-  SVAR(SF_CODEC | SF_NB16, "codec (16-row operand)"), SVAR(SF_CODEC, "codec"), SVAR(SF_ALL, "all"),
-  // after "all", so every program without the per-row solver runs on the variant it ran on before these existed
-  SVAR(SF_SAMP | SF_DPMROW | SF_NB16, "sampler, per-row solver (16-row operand)"), SVAR(SF_SAMP | SF_DPMROW, "sampler, per-row solver")};
+  SVAR(SF_CODEC | SF_NB16, "codec (16-row operand)"), SVAR(SF_CODEC, "codec"), SVAR(SF_ALL, "all")};
 #undef SVAR
-constexpr int N_STREAM_VARIANTS = 10;
+constexpr int N_STREAM_VARIANTS = 8;
 constexpr int STREAM_VARIANT_ALL = 7;
 
 constexpr int ST_MIN_RING = 3;    // ring slots a program must keep: a linear stage whose operand region leaves fewer is split along K
@@ -544,9 +541,8 @@ static int finish_stream(StreamBuilder& b, vv_ctx::StreamProg* pr) {
     feat |= (1u << o.pro) | (1u << (16 + o.kind)) | (1u << (24 + o.alpha_kind));
     if ((o.kind == SK_ATTN || o.pro == SP_COMBINE || o.rope_rows > 0) && o.att.hd != 128) hd128 = false;
   }
-  if (b.dpm_rows) feat |= SF_DPMROW;
   pr->variant = STREAM_VARIANT_ALL;
-  if (!getenv("VV_STREAM_GENERIC") || b.dpm_rows)          // the per-row solver exists only in its own variants
+  if (!getenv("VV_STREAM_GENERIC"))
     for (int v = 0; v < N_STREAM_VARIANTS; ++v)
       if ((feat & ~STREAM_VARIANTS[v].feat) == 0 && (hd128 || !(STREAM_VARIANTS[v].feat & SF_HD128)) && (nb16 || !(STREAM_VARIANTS[v].feat & SF_NB16)) &&
           !(getenv("VV_STREAM_NO_NB16") && (STREAM_VARIANTS[v].feat & SF_NB16))) { pr->variant = v; break; }
@@ -1096,7 +1092,10 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     *hb += (int64_t)2 * H * H * 2;
     drop(c, h + ".final_layer.adaLN_modulation.1.weight");
     const int NS = std::max(d.max_diffusion_steps, 1);
-    RET(dmalloc(c, &c->temb, (size_t)NS * H));
+    RET(dmalloc(c, &c->row_coef, (size_t)NS * B));
+    RET(dmalloc(c, &c->row_cfg, (size_t)B));
+    RET(dmalloc(c, &c->row_temb, (size_t)B * NS * H));
+    c->row_sde.assign(B, 0);
     RET(dmalloc(c, &c->tfreqs, 128));
     std::vector<float> fr(128);
     for (int j = 0; j < 128; ++j) fr[j] = expf((-9.210340371976184f * (float)j) / 128.0f);
@@ -1106,7 +1105,6 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
     RET(dmalloc(c, &c->s_condp, (size_t)M2 * H));
     RET(dmalloc(c, &c->s_call, (size_t)NS * M2 * H));
     RET(dmalloc(c, &c->s_mod, (size_t)NS * M2 * modrows));
-    RET(dmalloc(c, &c->cfg_dev, 4));
     RET(dmalloc(c, &c->gridbar, 2));
     RET(dmalloc(c, &c->st_bar, 32));
     if (getenv("VV_STREAM_TRACE")) {
@@ -1588,13 +1586,6 @@ extern "C" int vv_embed_tokens(vv_ctx* c, const int32_t* tokens_host, int n, flo
 // ------------------------------------------------------------------------------------------------
 // a-4: diffusion sampler
 // ------------------------------------------------------------------------------------------------
-static int set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, const float* coef, int ncol, void* stream);
-extern "C" int vv_set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, const float* coef, void* stream) {
-  return set_diffusion_steps(c, n_steps, timesteps, coef, 6, stream);
-}
-extern "C" int vv_set_diffusion_steps_sde(vv_ctx* c, int n_steps, const float* timesteps, const float* coef7, void* stream) {
-  return set_diffusion_steps(c, n_steps, timesteps, coef7, 7, stream);
-}
 extern "C" int vv_set_step_noise(vv_ctx* c, const float* step_noise) {
   if (!c) return fail(VV_ERR_INVALID, "null ctx");
   if (c->step_noise != step_noise) {            // captured graphs hold the old pointer
@@ -1603,76 +1594,101 @@ extern "C" int vv_set_step_noise(vv_ctx* c, const float* step_noise) {
   c->step_noise = step_noise;
   return 0;
 }
-static int set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, const float* coef, int ncol, void* stream) {
-  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  if (n_steps < 1 || n_steps > c->d.max_diffusion_steps) return fail(VV_ERR_INVALID, "n_steps %d outside [1,%d]", n_steps, c->d.max_diffusion_steps);
-  CK(cudaSetDevice(c->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  const int H = c->d.hidden_size;
-  std::vector<DpmCoef> cf(n_steps);
-  for (int i = 0; i < n_steps; ++i) {
-    cf[i].a0 = coef[i * ncol + 0]; cf[i].s0 = coef[i * ncol + 1]; cf[i].ks = coef[i * ncol + 2]; cf[i].kx = coef[i * ncol + 3];
-    cf[i].rinv = coef[i * ncol + 4]; cf[i].order = (int)coef[i * ncol + 5]; cf[i].kn = ncol == 7 ? coef[i * ncol + 6] : 0.f;
-  }
-  c->sde = (ncol == 7);
-  c->coef_host = cf;
-  c->coef_version++;
-  CK(cudaStreamSynchronize(s));
-  float* tdev = c->s_t1;   // reuse as staging for the timesteps (n floats) before it is overwritten below
-  CK(cudaMemcpy(tdev, timesteps, sizeof(float) * n_steps, cudaMemcpyHostToDevice));
-  timestep_feat_kernel<<<n_steps, 256, 0, s>>>(tdev, c->tfreqs, c->s_tfeat, n_steps);
-  CKL();
-  CK(cudaStreamSynchronize(s));
-  L l{c, s};
-  GemvP p = mk(c->h_t0, nullptr, c->s_tfeat, 256, c->s_t1, H, n_steps, H, 256);
-  p.epi = EPI_SILU;
-  RET(linear(l, p, c->temb_info[0]));
-  p = mk(c->h_t2, nullptr, c->s_t1, H, c->temb, H, n_steps, H, H);
-  RET(linear(l, p, c->temb_info[1]));
-  CK(cudaStreamSynchronize(s));
-  c->n_steps = n_steps;
-  // programs captured with another step count are stale
-  drop_graphs(c, {"tail:", "diff:", "frame:"});
-  return 0;
+
+// p[0 .. n) = v
+__global__ void set_float_kernel(float* p, float v, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) p[i] = v;
 }
 
-__global__ void set_float_kernel(float* p, float v) { *p = v; }
-
-// ---- per-row sampler settings: a queue of requests mixes step counts, solvers and CFG scales in one batch.  Every row runs row_nmax solver
-// steps per frame; a row with n < row_nmax steps runs row_nmax - n identity steps (ks = 1, kx = 0, s0 = 0, kn = 0, order 1) and then its own
-// n steps, whose first is first-order as in a solo run.  The identity steps are conditioned on the row's first timestep, so the head sees
-// finite inputs there (0 * NaN would survive z' = ks z - kx x0).  Settings live in device tables: changing them rebuilds no program and
-// captures no graph.
-extern "C" int vv_sampler_per_row(vv_ctx* c, int n_max, void* stream) {
-  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  if (n_max < 0 || n_max > c->d.max_diffusion_steps) return fail(VV_ERR_INVALID, "n_max %d outside [0,%d]", n_max, c->d.max_diffusion_steps);
-  CK(cudaSetDevice(c->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  const int B = c->d.max_batch, NS = std::max(c->d.max_diffusion_steps, 1), H = c->d.hidden_size;
-  if (n_max > 0) {
-    if (!c->row_coef) {
-      RET(dmalloc(c, &c->row_coef, (size_t)NS * B));
-      RET(dmalloc(c, &c->row_cfg, (size_t)B));
-      RET(dmalloc(c, &c->row_temb, (size_t)B * NS * H));
-    }
-    // every row starts as identity steps on a zero timestep embedding with CFG scale 1: finite, and its latent is its noise
-    std::vector<DpmCoef> id((size_t)n_max * B, DpmCoef{0.f, 0.f, 1.f, 0.f, 0.f, 1, 0.f});
-    std::vector<float> one(B, 1.f);
-    CK(cudaMemcpyAsync(c->row_coef, id.data(), id.size() * sizeof(DpmCoef), cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(c->row_cfg, one.data(), B * sizeof(float), cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(c->row_temb, 0, (size_t)B * n_max * H * sizeof(float), s));
-    CK(cudaStreamSynchronize(s));        // the host tables above are about to go out of scope
-  }
-  c->row_sde.assign(B, 0);
+// The sampler's settings live in device tables, one column per row: changing them rebuilds no program and captures no graph, only a
+// change of row_nmax (the program's step count and the tables' layout) does.
+static int set_nmax(vv_ctx* c, int n_max) {
   if (n_max != c->row_nmax) drop_graphs(c, {"tail:", "diff:", "frame:"});
   c->row_nmax = n_max;
   return 0;
 }
 
+// One solver's settings of n_steps steps: coef[n_steps][ncol] (ncol 6: dpmsolver++, 7: sde-dpmsolver++ with kn) into cf[0, n_steps), and
+// the timestep embeddings t_embedder(timesteps) [n_steps][H] into temb (stream order).  info (optional): {kernel, split-K} of the two
+// t-embedder linears.  Every caller runs these kernels with this row count, so a row's embeddings are bit-identical whoever wrote them.
+static int solver_settings(vv_ctx* c, int n_steps, const float* timesteps, const float* coef, int ncol, DpmCoef* cf, float* temb,
+                           cudaStream_t s, int32_t (*info)[2] = nullptr) {
+  for (int i = 0; i < n_steps; ++i) {
+    DpmCoef& k = cf[i];
+    k.a0 = coef[i * ncol + 0]; k.s0 = coef[i * ncol + 1]; k.ks = coef[i * ncol + 2]; k.kx = coef[i * ncol + 3];
+    k.rinv = coef[i * ncol + 4]; k.order = (int)coef[i * ncol + 5]; k.kn = ncol == 7 ? coef[i * ncol + 6] : 0.f;
+  }
+  const int H = c->d.hidden_size;
+  float* tdev = c->s_t1;   // staging for the timesteps, overwritten below (stream order)
+  CK(cudaMemcpyAsync(tdev, timesteps, sizeof(float) * n_steps, cudaMemcpyHostToDevice, s));
+  timestep_feat_kernel<<<n_steps, 256, 0, s>>>(tdev, c->tfreqs, c->s_tfeat, n_steps);
+  CKL();
+  c->launches++;
+  L l{c, s};
+  GemvP p = mk(c->h_t0, nullptr, c->s_tfeat, 256, c->s_t1, H, n_steps, H, 256);
+  p.epi = EPI_SILU;
+  RET(linear(l, p, info ? info[0] : nullptr));
+  p = mk(c->h_t2, nullptr, c->s_t1, H, temb, H, n_steps, H, H);
+  RET(linear(l, p, info ? info[1] : nullptr));
+  return 0;
+}
+
+// every row gets the same n_steps steps; the CFG scale is the sampling call's (set_cfg)
+static int set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, const float* coef, int ncol, void* stream) {
+  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  if (n_steps < 1 || n_steps > c->d.max_diffusion_steps) return fail(VV_ERR_INVALID, "n_steps %d outside [1,%d]", n_steps, c->d.max_diffusion_steps);
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int B = c->d.max_batch, H = c->d.hidden_size;
+  std::vector<DpmCoef> cf(n_steps), all((size_t)n_steps * B);
+  RET(solver_settings(c, n_steps, timesteps, coef, ncol, cf.data(), c->row_temb, s, c->temb_info));     // row 0's slice
+  for (int i = 0; i < n_steps; ++i)
+    for (int b = 0; b < B; ++b) all[(size_t)i * B + b] = cf[i];
+  CK(cudaMemcpyAsync(c->row_coef, all.data(), all.size() * sizeof(DpmCoef), cudaMemcpyHostToDevice, s));
+  for (int b = 1; b < B; ++b)
+    CK(cudaMemcpyAsync(c->row_temb + (size_t)b * n_steps * H, c->row_temb, (size_t)n_steps * H * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  CK(cudaStreamSynchronize(s));          // the host tables go out of scope
+  c->row_sde.assign(B, ncol == 7);
+  c->uniform = true;
+  c->cfg_last = NAN;                     // the CFG entries hold whatever the last per-row settings left
+  return set_nmax(c, n_steps);
+}
+extern "C" int vv_set_diffusion_steps(vv_ctx* c, int n_steps, const float* timesteps, const float* coef, void* stream) {
+  return set_diffusion_steps(c, n_steps, timesteps, coef, 6, stream);
+}
+extern "C" int vv_set_diffusion_steps_sde(vv_ctx* c, int n_steps, const float* timesteps, const float* coef7, void* stream) {
+  return set_diffusion_steps(c, n_steps, timesteps, coef7, 7, stream);
+}
+
+// ---- per-row sampler settings: a queue of requests mixes step counts, solvers and CFG scales in one batch.  Every row runs row_nmax solver
+// steps per frame; a row with n < row_nmax steps runs row_nmax - n identity steps (ks = 1, kx = 0, s0 = 0, kn = 0, order 1) and then its own
+// n steps, whose first is first-order as in a solo run.  The identity steps are conditioned on the row's first timestep, so the head sees
+// finite inputs there (0 * NaN would survive z' = ks z - kx x0).
+extern "C" int vv_sampler_per_row(vv_ctx* c, int n_max, void* stream) {
+  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  if (n_max < 0 || n_max > c->d.max_diffusion_steps) return fail(VV_ERR_INVALID, "n_max %d outside [0,%d]", n_max, c->d.max_diffusion_steps);
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int B = c->d.max_batch, H = c->d.hidden_size;
+  if (n_max > 0) {
+    // every row starts as identity steps on a zero timestep embedding with CFG scale 1: finite, and its latent is its noise
+    std::vector<DpmCoef> id((size_t)n_max * B, DpmCoef{0.f, 0.f, 1.f, 0.f, 0.f, 1, 0.f});
+    CK(cudaMemcpyAsync(c->row_coef, id.data(), id.size() * sizeof(DpmCoef), cudaMemcpyHostToDevice, s));
+    set_float_kernel<<<1, 32, 0, s>>>(c->row_cfg, 1.f, B);
+    CKL();
+    c->launches++;
+    CK(cudaMemsetAsync(c->row_temb, 0, (size_t)B * n_max * H * sizeof(float), s));
+    CK(cudaStreamSynchronize(s));        // the host table above is about to go out of scope
+  }
+  c->row_sde.assign(B, 0);
+  c->uniform = false;
+  return set_nmax(c, n_max);
+}
+
 extern "C" int vv_set_row_sampler(vv_ctx* c, int row, int n_steps, const float* timesteps, const float* coef, int ncol, float cfg_scale,
                                   void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
-  if (c->row_nmax < 1) return fail(VV_ERR_STATE, "vv_set_row_sampler: per-row mode is off (vv_sampler_per_row)");
+  if (c->row_nmax < 1 || c->uniform) return fail(VV_ERR_STATE, "vv_set_row_sampler: per-row mode is off (vv_sampler_per_row)");
   if (row < 0 || row >= c->d.max_batch) return fail(VV_ERR_INVALID, "vv_set_row_sampler: bad row %d", row);
   if (n_steps < 1 || n_steps > c->row_nmax) return fail(VV_ERR_INVALID, "vv_set_row_sampler: n_steps %d outside [1,%d]", n_steps, c->row_nmax);
   if (ncol != 6 && ncol != 7) return fail(VV_ERR_INVALID, "vv_set_row_sampler: ncol %d (6: dpmsolver++, 7: sde-dpmsolver++)", ncol);
@@ -1681,42 +1697,32 @@ extern "C" int vv_set_row_sampler(vv_ctx* c, int row, int n_steps, const float* 
   cudaStream_t s = (cudaStream_t)stream;
   const int B = c->d.max_batch, N = c->row_nmax, H = c->d.hidden_size, pad = N - n_steps;
   std::vector<DpmCoef> cf(N, DpmCoef{0.f, 0.f, 1.f, 0.f, 0.f, 1, 0.f});
-  for (int i = 0; i < n_steps; ++i) {
-    DpmCoef& k = cf[pad + i];
-    k.a0 = coef[i * ncol + 0]; k.s0 = coef[i * ncol + 1]; k.ks = coef[i * ncol + 2]; k.kx = coef[i * ncol + 3];
-    k.rinv = coef[i * ncol + 4]; k.order = (int)coef[i * ncol + 5]; k.kn = ncol == 7 ? coef[i * ncol + 6] : 0.f;
-  }
-  CK(cudaMemcpy2DAsync(c->row_coef + row, (size_t)B * sizeof(DpmCoef), cf.data(), sizeof(DpmCoef), sizeof(DpmCoef), N, cudaMemcpyHostToDevice, s));
-  set_float_kernel<<<1, 1, 0, s>>>(c->row_cfg + row, cfg_scale);
-  CKL();
-  // the row's timestep embeddings: the kernels and row count (M = n_steps) of vv_set_diffusion_steps, so the slice is bit-identical to a
-  // solo run's table
-  float* tdev = c->s_t1;   // staging for the timesteps, overwritten below (stream order)
-  CK(cudaMemcpyAsync(tdev, timesteps, sizeof(float) * n_steps, cudaMemcpyHostToDevice, s));
-  timestep_feat_kernel<<<n_steps, 256, 0, s>>>(tdev, c->tfreqs, c->s_tfeat, n_steps);
-  CKL();
   float* dst = c->row_temb + (size_t)row * N * H;
-  L l{c, s};
-  GemvP p = mk(c->h_t0, nullptr, c->s_tfeat, 256, c->s_t1, H, n_steps, H, 256);
-  p.epi = EPI_SILU;
-  RET(linear(l, p));
-  p = mk(c->h_t2, nullptr, c->s_t1, H, dst + (size_t)pad * H, H, n_steps, H, H);
-  RET(linear(l, p));
+  RET(solver_settings(c, n_steps, timesteps, coef, ncol, cf.data() + pad, dst + (size_t)pad * H, s));
+  CK(cudaMemcpy2DAsync(c->row_coef + row, (size_t)B * sizeof(DpmCoef), cf.data(), sizeof(DpmCoef), sizeof(DpmCoef), N, cudaMemcpyHostToDevice, s));
+  set_float_kernel<<<1, 32, 0, s>>>(c->row_cfg + row, cfg_scale, 1);
+  CKL();
+  c->launches++;
   for (int i = 0; i < pad; ++i)
     CK(cudaMemcpyAsync(dst + (size_t)i * H, dst + (size_t)pad * H, (size_t)H * sizeof(float), cudaMemcpyDeviceToDevice, s));
   CK(cudaStreamSynchronize(s));          // cf goes out of scope
   c->row_sde[row] = ncol == 7;
-  c->launches += 2;
   return 0;
 }
-// the CFG scale is read from device memory by the solver kernels, so one captured graph serves every value (a service with a
-// user-controlled cfg_scale would otherwise capture and keep one frame-tail graph per distinct float)
+// uniform settings: the sampling call's CFG scale goes to every row.  The solver kernels read it from device memory, so one captured graph
+// serves every value (a service with a user-controlled cfg_scale would otherwise capture and keep one frame-tail graph per distinct float).
+// Per-row settings carry their own scales and ignore the call's.
 static int set_cfg(vv_ctx* c, float cfg, cudaStream_t s) {
-  if (memcmp(&cfg, &c->cfg_last, sizeof(float)) == 0) return 0;
-  set_float_kernel<<<1, 1, 0, s>>>(c->cfg_dev, cfg);
+  if (!c->uniform || memcmp(&cfg, &c->cfg_last, sizeof(float)) == 0) return 0;
+  set_float_kernel<<<1, 32, 0, s>>>(c->row_cfg, cfg, c->d.max_batch);
   CKL();
   c->launches++;
   c->cfg_last = cfg;
+  return 0;
+}
+static int check_step_noise(const vv_ctx* c) {
+  if (!c->step_noise && std::find(c->row_sde.begin(), c->row_sde.end(), 1) != c->row_sde.end())
+    return fail(VV_ERR_STATE, "sde-dpmsolver++ needs vv_set_step_noise before sampling");
   return 0;
 }
 
@@ -1727,16 +1733,13 @@ static int set_cfg(vv_ctx* c, float cfg, cudaStream_t s) {
 // 1 + i (L + 2): head layer li = 0 .. L-1 (gate/up + down), the final layer, proj(i).  sampler_build emits blocks [blk0, blk1) only.  Every
 // value one block hands to the next lives in global memory (s_hx, the gu double buffer, s_v, the s_z / s_x0 parity buffers, s_mod) and the
 // zero-fill jobs ride on earlier stages, so the blocks launched one after another compute what the whole program does (vv_debug_sampler_taps).
-static int samp_steps(const vv_ctx* c) { return c->row_nmax > 0 ? c->row_nmax : c->n_steps; }
-static int sampler_blocks(const vv_ctx* c) { return 1 + samp_steps(c) * (c->d.head_layers + 2); }
+static int sampler_blocks(const vv_ctx* c) { return 1 + c->row_nmax * (c->d.head_layers + 2); }
 static int sampler_build(StreamBuilder& b, const float* noise, float* latent_out, int blk0, int blk1) {
   vv_ctx* c = b.c;
   const auto& d = c->d;
-  const int H = d.hidden_size, F = d.head_ffn_dim, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = samp_steps(c);
-  const bool rows = c->row_nmax > 0;
+  const int H = d.hidden_size, F = d.head_ffn_dim, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = c->row_nmax;
   const long long modld = (long long)(3 * LH + 2) * H;
   auto in = [&](int blk) { return blk >= blk0 && blk < blk1; };
-  b.dpm_rows = rows;
   auto dpm = [&](int i) {
     SDpm o;
     memset(&o, 0, sizeof o);
@@ -1745,11 +1748,8 @@ static int sampler_build(StreamBuilder& b, const float* noise, float* latent_out
       o.z_in = c->s_z + (size_t)(i & 1) * B * 64; o.z_out = c->s_z + (size_t)((i + 1) & 1) * B * 64;
       o.x0_in = c->s_x0 + (size_t)(i & 1) * B * 64; o.x0_out = c->s_x0 + (size_t)((i + 1) & 1) * B * 64;
     }
-    o.v = c->s_v; o.noise = noise; o.cfg_p = rows ? c->row_cfg : c->cfg_dev;
-    o.step_noise = (rows || c->sde) ? c->step_noise : nullptr;
+    o.v = c->s_v; o.noise = noise; o.cfg_p = c->row_cfg; o.step_noise = c->step_noise; o.rows = c->row_coef;
     o.latent_out = (i == N - 1) ? latent_out : nullptr; o.step = i; o.B = B;
-    if (rows) o.rows = c->row_coef;
-    else if (i >= 0) o.c = c->coef_host[i];
     return o;
   };
   auto proj = [&](int i, bool sync) -> int {       // x = noisy_images_proj(z'), z' = solver update of step i (i = -1: the initial noise)
@@ -1790,12 +1790,8 @@ static int sampler_build(StreamBuilder& b, const float* noise, float* latent_out
   return 0;
 }
 static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out, const vv_ctx::StreamProg** out) {
-  char key[256];
-  if (c->row_nmax > 0)             // per-row mode: coefficients and CFG scales are read from device tables, only the step count is baked in
-    snprintf(key, sizeof key, "samp:%p:%p:rows%d:%p", (const void*)noise, (void*)latent_out, c->row_nmax, (const void*)c->step_noise);
-  else
-    snprintf(key, sizeof key, "samp:%p:%p:%d:%d:%p:%d", (const void*)noise, (void*)latent_out, c->n_steps, (int)c->sde, (const void*)c->step_noise,
-             c->coef_version);     // solver coefficients are baked into the program
+  char key[256];                   // coefficients and CFG scales are read from device tables, only the step count is baked in
+  snprintf(key, sizeof key, "samp:%p:%p:%d:%p", (const void*)noise, (void*)latent_out, c->row_nmax, (const void*)c->step_noise);
   auto it = c->sprogs.find(key);
   if (it != c->sprogs.end()) { *out = &it->second; return 0; }
   StreamBuilder b(c);
@@ -1812,21 +1808,16 @@ static int sampler_stream_prog(vv_ctx* c, const float* noise, float* latent_out,
 static int diffusion_preamble(const L& l, const float* cond, int32_t* info_cond = nullptr, int32_t* info_mod = nullptr) {
   vv_ctx* c = l.c;
   const auto& d = c->d;
-  const int H = d.hidden_size, M = 2 * d.max_batch, LH = d.head_layers, N = samp_steps(c);
+  const int H = d.hidden_size, M = 2 * d.max_batch, LH = d.head_layers, N = c->row_nmax;
   if (N < 1) return fail(VV_ERR_STATE, "vv_set_diffusion_steps not called");
   const int modld = (3 * LH + 2) * H;
-  const bool rows = c->row_nmax > 0;
-  const bool sde = rows ? std::find(c->row_sde.begin(), c->row_sde.end(), 1) != c->row_sde.end() : c->sde;
-  if (sde && !c->step_noise) return fail(VV_ERR_STATE, "sde-dpmsolver++ needs vv_set_step_noise before sampling");
+  RET(check_step_noise(c));
   GemvP p = mk(c->h_cond, nullptr, cond, H, c->s_condp, H, M, H, H);
   RET(linear(l, p, info_cond));
   {
     const long long n = (long long)N * M * H;
-    if (rows)
-      CK(launch_k(l, head_cond_prep_rows_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, c->s_condp, c->row_temb, c->s_call, N, M,
-                  d.max_batch, H));
-    else
-      CK(launch_k(l, head_cond_prep_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, c->s_condp, c->temb, c->s_call, N, M, H));
+    CK(launch_k(l, head_cond_prep_rows_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, c->s_condp, c->row_temb, c->s_call, N, M,
+                d.max_batch, H));
   }
   // AdaLN modulation of ALL steps and layers in one tensor-core GEMM: c_all [N*M, H] x W_mod^T -> [N*M, (3L+2)H].
   // (the reference recomputes Linear(silu(c)) inside every head call, diffusion_head.py:159, 185; c depends only on (cond, t_i))
@@ -1845,7 +1836,7 @@ extern "C" int vv_diffusion_sample(vv_ctx* c, const float* cond, const float* no
   (void)active;   // rows are independent; inactive rows are computed and ignored (static shapes keep the program graph-replayable)
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
   CK(cudaSetDevice(c->device));
-  if (c->row_nmax == 0) RET(set_cfg(c, cfg, (cudaStream_t)stream));     // per-row mode: the scales come from vv_set_row_sampler
+  RET(set_cfg(c, cfg, (cudaStream_t)stream));
   char key[256];
   snprintf(key, sizeof key, "diff:%p:%p:%p", (const void*)cond, (const void*)noise, (void*)latent_out);
   const vv_ctx::StreamProg* sprog;      // built outside stream capture (it allocates and copies)
@@ -1859,10 +1850,10 @@ enum { STAP_THID = 0, STAP_TEMB, STAP_COND, STAP_MOD, STAP_LAYER, STAP_V, STAP_Z
 struct SampTap { int kind, step, layer, rows, cols; const float* src; int block; };
 static void sampler_tap_plan(const vv_ctx* c, float* latent_out, std::vector<SampTap>* plan) {
   const auto& d = c->d;
-  const int H = d.hidden_size, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = c->n_steps, modld = (3 * LH + 2) * H;
+  const int H = d.hidden_size, B = d.max_batch, M = 2 * B, LH = d.head_layers, N = c->row_nmax, modld = (3 * LH + 2) * H;
   plan->clear();
   plan->push_back({STAP_THID, -1, -1, N, H, c->s_t1, -1});
-  plan->push_back({STAP_TEMB, -1, -1, N, H, c->temb, -1});
+  plan->push_back({STAP_TEMB, -1, -1, N, H, c->row_temb, -1});     // row 0's slice (every row's, vv_set_diffusion_steps)
   plan->push_back({STAP_COND, -1, -1, M, H, c->s_condp, -1});
   plan->push_back({STAP_MOD, -1, -1, N * M, modld, c->s_mod, -1});
   auto proj = [&](int i, int blk) {             // proj(i) writes z_{i+1} and x0_i into parity slot (i + 1) & 1 (i = -1: slot 0)
@@ -1887,14 +1878,13 @@ static bool same_stage(const SOp& a, const SOp& b) {
          a.ldy == b.ldy && a.alpha_kind == b.alpha_kind && a.alpha == b.alpha && a.store == b.store && a.init_dst == b.init_dst &&
          a.init_n == b.init_n && a.dpm.z_in == b.dpm.z_in && a.dpm.z_out == b.dpm.z_out && a.dpm.x0_in == b.dpm.x0_in &&
          a.dpm.x0_out == b.dpm.x0_out && a.dpm.v == b.dpm.v && a.dpm.noise == b.dpm.noise && a.dpm.step_noise == b.dpm.step_noise &&
-         a.dpm.latent_out == b.dpm.latent_out && a.dpm.step == b.dpm.step && memcmp(&a.dpm.c, &b.dpm.c, sizeof a.dpm.c) == 0;
+         a.dpm.latent_out == b.dpm.latent_out && a.dpm.step == b.dpm.step && a.dpm.cfg_p == b.dpm.cfg_p && a.dpm.rows == b.dpm.rows;
 }
 extern "C" int vv_debug_sampler_taps(vv_ctx* c, const float* cond, const float* noise, float cfg, float* latent_out, float* taps,
                                      int64_t taps_floats, int32_t* meta, void* stream) {
   if (!c) return fail(VV_ERR_INVALID, "null ctx");
   if (!c->finalized) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: not finalized");
-  if (c->n_steps < 1) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: vv_set_diffusion_steps not called");
-  if (c->row_nmax > 0) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: global sampler mode only (vv_sampler_per_row(ctx, 0, ...))");
+  if (!c->uniform) return fail(VV_ERR_STATE, "vv_debug_sampler_taps: needs the settings of vv_set_diffusion_steps (not per-row ones)");
   std::vector<SampTap> plan;
   sampler_tap_plan(c, latent_out, &plan);
   const int n = (int)plan.size();
@@ -1907,7 +1897,7 @@ extern "C" int vv_debug_sampler_taps(vv_ctx* c, const float* cond, const float* 
   if (!taps) return n;
   if (taps_floats < need) return fail(VV_ERR_INVALID, "vv_debug_sampler_taps: %lld floats of tap space, the sampler needs %lld", (long long)taps_floats, need);
   if (!cond || !noise || !latent_out) return fail(VV_ERR_INVALID, "vv_debug_sampler_taps: null condition, noise or latent");
-  if (c->sde && !c->step_noise) return fail(VV_ERR_STATE, "sde-dpmsolver++ needs vv_set_step_noise before sampling");
+  RET(check_step_noise(c));
   CK(cudaSetDevice(c->device));
   cudaStream_t s = (cudaStream_t)stream;
   // production's own program (cached under its production key, as vv_diffusion_sample would): every block must run on its kernel variant
@@ -2377,7 +2367,7 @@ extern "C" int vv_frame_tail(vv_ctx* c, const float* hidden, const float* noise,
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
   CK(cudaSetDevice(c->device));
   char key[320];
-  if (c->row_nmax == 0) RET(set_cfg(c, cfg, (cudaStream_t)stream));     // per-row mode: the scales come from vv_set_row_sampler
+  RET(set_cfg(c, cfg, (cudaStream_t)stream));
   snprintf(key, sizeof key, "tail:%p:%p:%p:%p:%p:%p", (const void*)hidden, (const void*)noise, (const void*)active, (void*)latent_out,
            (void*)audio_out, (void*)embeds);
   const vv_ctx::StreamProg *sprog, *front, *back; int nf; float* fx;

@@ -106,18 +106,16 @@ enum SAlpha { SA_ONE = 0, SA_GATE = 1 /* alpha[m][n], row stride lda */, SA_GAMM
 // B-operand row m = z'[m mod B].  Rows b (conditional) and B+b (unconditional) of the head output v give
 //   v = v_u + s (v_c - v_u); x0 = a0 z - s0 v; z' = ks z - kx x0 [- 0.5 kx rinv (x0 - x0_prev)] [+ kn * step_noise[step]]
 // (modeling_vibevoice_inference.py:703-709 + schedule/dpm_solver.py:581-584, 669-677, 738-764; sde-dpmsolver++, dpm_solver.py:680-686 /
-// 785-793: same two forms with other ks / kx plus the variance-noise term; step_noise is [n_steps][B][64] or nullptr for the ODE solver).
-// step = -1: z' = the initial noise.
-// Per-row mode (programs on the SF_DPMROW variants, vv_sampler_per_row): s and the coefficients are per sample -- cfg_p is cfg[B] and
-// the coefficients of sample b come from rows[step][b]; a row with fewer steps than the program runs identity steps (ks = 1, kx = 0) first.
+// 785-793: same two forms with other ks / kx plus the variance-noise term; step_noise is [n_steps][B][64], nullptr until
+// vv_set_step_noise binds it).  step = -1: z' = the initial noise.
+// s and the coefficients are per sample: cfg_p is cfg[B] and the coefficients of sample b come from rows[step][b]; a row with fewer steps
+// than the program runs identity steps (ks = 1, kx = 0, kn = 0) first (vv_set_row_sampler).
 struct SDpm {
   const float* z_in; float* z_out; const float* x0_in; float* x0_out; const float* v; const float* noise;
   const float* cfg_p; const float* step_noise; float* latent_out;
   int step, B;
-  union {
-    DpmCoef c;              // coefficients of this step, by value (no dependent loads on the critical path)
-    const DpmCoef* rows;    // per-row mode: [n_steps][B] device table
-  };
+  const DpmCoef* rows;      // [n_steps][B] device table
+  unsigned char pad_[24];   // keeps SOp at its size: a smaller descriptor changes ptxas' register allocation of every kernel variant
 };
 
 // Decode attention as a stage of the stream (SK_ATTN), and its split-partial merge as the prologue of the o-projection (SP_COMBINE).
@@ -420,8 +418,6 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
 #define ATT_HD(a) ((((FEAT >> 30) & 1u) != 0u) ? 128 : (a).hd)
 // bit 29: every linear stage of the program has a 16-row activation operand (M <= 8 rows: one prompt per GPU) -> compile-time nB
 #define OP_NB(o) ((((FEAT >> 29) & 1u) != 0u) ? 16 : (o).nB)
-// bit 28: SP_DPM takes its CFG scale and solver coefficients per sample from device tables (SDpm, per-row mode)
-  constexpr bool DPM_ROWS = ((FEAT >> 28) & 1u) != 0u;
   extern __shared__ unsigned char st_raw[];
   __shared__ unsigned long long full_bar[ST_MAX_STAGES], empty_bar[ST_MAX_STAGES];
   __shared__ float s_red[4][8];
@@ -1138,8 +1134,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stream_kernel(SParams P) {
           if (d.step < 0) {
             zn = ldcg1(d.noise + i);
           } else {
-            const DpmCoef c = DPM_ROWS ? d.rows[(size_t)d.step * d.B + b] : d.c;
-            const float cfg = DPM_ROWS ? ldcg1(d.cfg_p + b) : *d.cfg_p;
+            const DpmCoef c = d.rows[(size_t)d.step * d.B + b];
+            const float cfg = ldcg1(d.cfg_p + b);
             const float vc = ldcg1(d.v + (size_t)b * 64 + e), vu = ldcg1(d.v + (size_t)(d.B + b) * 64 + e);
             const float vv_ = vu + cfg * (vc - vu);
             const float zo = ldcg1(d.z_in + i);

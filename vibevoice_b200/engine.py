@@ -85,6 +85,8 @@ class Engine:
             self.latent = torch.zeros(B, 64, dtype=torch.float32, device=dev)
             self.audio = torch.zeros(B, 3200, dtype=torch.float32, device=dev)
             self.feat = torch.zeros(B, config.semantic_vae_dim, dtype=torch.float32, device=dev)
+            # sde-dpmsolver++ variance noise [step][row][64] of every sampler setting (vv_set_step_noise, bound once in finalize)
+            self.step_noise = torch.zeros(max(max_diffusion_steps, 1), B, 64, dtype=torch.float32, device=dev)
         self.tokens_h = torch.zeros(B, dtype=torch.int32).pin_memory()
         self.logits_h = torch.zeros(B, len(self.valid_ids), dtype=torch.float32).pin_memory()
         self.noise_h = torch.zeros(B, 64, dtype=torch.float32).pin_memory()
@@ -92,7 +94,6 @@ class Engine:
         self.eos_d = torch.zeros(2, self.EOS_MAX_ROWS, dtype=torch.float32, device=dev)     # vv_eos_prob(_rows): probabilities, logits
         self.eos_h = torch.zeros(2, self.EOS_MAX_ROWS, dtype=torch.float32).pin_memory()
         self.n_steps = 0
-        self.step_noise = None
         self.scheduler = DPMSolverMultistepScheduler(
             num_train_timesteps=config.diffusion_head_config.ddpm_num_steps,
             beta_schedule=config.diffusion_head_config.ddpm_beta_schedule,
@@ -135,6 +136,7 @@ class Engine:
         if speech_scaling_factor is not None:
             N.check(self.lib.vv_set_speech_factors(self.h, float(speech_scaling_factor), float(speech_bias_factor)))
         N.check(self.lib.vv_finalize_weights(self.h), "vv_finalize_weights")
+        N.check(self.lib.vv_set_step_noise(self.h, C.c_void_p(self.step_noise.data_ptr())), "vv_set_step_noise")
         self.finalized = True
         # Qwen2RotaryEmbedding.inv_freq exactly as torch computes it (fp32)
         dc = self.config.decoder_config
@@ -401,30 +403,28 @@ class Engine:
         self.scheduler.set_timesteps(n_steps)
         ts = np.ascontiguousarray(self.scheduler.timesteps.numpy().astype(np.float32))
         coef = np.ascontiguousarray(self.scheduler.coef)
+        self._clear_step_noise()
         if self.sde:
-            if self.step_noise is None or self.step_noise.shape[0] < n_steps:
-                with torch.cuda.device(self.device):
-                    self.step_noise = torch.zeros(max(n_steps, 8), self.B, 64, dtype=torch.float32, device=self.device)
             N.check(self.lib.vv_set_diffusion_steps_sde(self.h, n_steps, N.iptr(ts), N.iptr(coef), self.s), "vv_set_diffusion_steps_sde")
-            N.check(self.lib.vv_set_step_noise(self.h, C.c_void_p(self.step_noise.data_ptr())), "vv_set_step_noise")
         else:
             N.check(self.lib.vv_set_diffusion_steps(self.h, n_steps, N.iptr(ts), N.iptr(coef), self.s), "vv_set_diffusion_steps")
         self.n_steps = n_steps
 
     def sampler_per_row(self, n_max: int):
-        """Switch the sampler to per-row settings with `n_max` solver steps per frame for every row (`vv_sampler_per_row`); 0 switches back
-        to the global settings of `set_diffusion_steps`, which are then rebuilt on its next call."""
+        """Switch the sampler to per-row settings with `n_max` solver steps per frame for every row (`vv_sampler_per_row`); 0 leaves the
+        sampler unset until the next `set_diffusion_steps`, which this forces to rebuild the tables for every row."""
         n_max = int(n_max)
-        if n_max > 0:
-            with torch.cuda.device(self.device):
-                self.row_step_noise = torch.zeros(n_max, self.B, 64, dtype=torch.float32, device=self.device)
-            N.check(self.lib.vv_set_step_noise(self.h, C.c_void_p(self.row_step_noise.data_ptr())), "vv_set_step_noise")
+        self._clear_step_noise()
         N.check(self.lib.vv_sampler_per_row(self.h, n_max, self.s), "vv_sampler_per_row")
         self.row_nmax = n_max
         self.row_steps = [n_max] * self.B
         if n_max == 0:
-            self.row_step_noise = None
-            self.n_steps = 0                          # the global tables (and step-noise binding) are set again on the next call
+            self.n_steps = 0
+
+    def _clear_step_noise(self):
+        """dpmsolver++ rows add 0 * step_noise: new settings start from a zero buffer, so nothing a previous setting left there counts."""
+        with torch.cuda.stream(self.stream):
+            self.step_noise.zero_()
 
     def set_row_sampler(self, row: int, n_steps: int, solver: str, cfg_scale: float):
         """Row `row` samples with `n_steps` steps of `solver` ("dpmsolver++" or "sde-dpmsolver++", on the engine scheduler's
@@ -441,7 +441,7 @@ class Engine:
         """sde-dpmsolver++ rows in per-row mode: noise [n_steps, 64] of row `row`'s own steps, which run last of the frame's n_max."""
         n = self.row_steps[row]
         with torch.cuda.stream(self.stream):
-            self.row_step_noise[self.row_nmax - n:, row].copy_(noise.to(self.device, torch.float32), non_blocking=True)
+            self.step_noise[self.row_nmax - n:self.row_nmax, row].copy_(noise.to(self.device, torch.float32), non_blocking=True)
 
     def kv_pages_free(self) -> int:
         return int(self.lib.vv_kv_pages_free(self.h))
