@@ -101,8 +101,24 @@ int vv_kv_write(vv_ctx* ctx, int seq, int layer, int64_t pos0, int64_t n_tokens,
                 const void* k_bf16, const void* v_bf16, void* stream);   /* prefill hand-off: [n_tokens, kv_heads, head_dim] */
 int vv_kv_delete_slot(vv_ctx* ctx, int seq, int64_t pos, void* stream);  /* forget ONE older entry: the last entry moves into its place (order is
                                                                            * irrelevant to attention); refresh_negative=False bookkeeping, :599-624 */
-int64_t vv_kv_pages_free(vv_ctx* ctx);
+int64_t vv_kv_pages_free(vv_ctx* ctx);          /* a page that several holders share counts once */
 int64_t vv_kv_pages_total(vv_ctx* ctx);
+
+/* ---- shared prefixes: whole pages of K/V that several sequences read, one copy in the pool ---------------------------------------- *
+ * Pages are reference-counted; a page returns to the free list when its last holder (sequence or prefix handle) lets go.  A sequence's
+ * positions below its shared length (the prefix it was attached to, or the prefix it was the source of) are immutable: vv_kv_write,
+ * vv_lm_prefill / vv_debug_prefill_taps and vv_kv_delete_slot refuse them with VV_ERR_INVALID and launch nothing, and vv_kv_set_len
+ * accepts 0 (which drops the sequence's references) or a length at or above the shared one.  Only whole pages are shared, so the next
+ * entry of a sequence always lands in a page of its own.  vv_kv_init drops every prefix; handles issued before it are invalid. */
+int vv_kv_prefix_create(vv_ctx* ctx, int seq, int64_t n_tokens, int* handle);  /* n_tokens: positive multiple of 64, <= kv_len(seq); the
+                                                                                  handle references the first n_tokens/64 pages of seq */
+int vv_kv_prefix_attach(vv_ctx* ctx, int handle, int seq, void* stream);       /* seq with kv_len 0 -> page-table entries [0, n/64) become
+                                                                                  the prefix's pages, kv_len = n; nothing is copied */
+int vv_kv_prefix_release(vv_ctx* ctx, int handle);
+int64_t vv_kv_prefix_tokens(vv_ctx* ctx, int handle);                          /* n_tokens of a live handle, else -1 (a query: no error
+                                                                                  message is recorded) */
+int64_t vv_kv_seq_pages(vv_ctx* ctx, int seq);                                 /* pages seq holds, shared ones included; -1 for a bad seq
+                                                                                  or before vv_kv_init */
 
 /* ---- a-3: LLM decode step for pos+neg rows in ONE weight pass ---------------------------------- *
  * replaces self(**model_inputs) at :480-482 and the negative forward at :583-585.

@@ -11,6 +11,15 @@ warm-up pass.  A second queue pass mixes step counts (5 / 10 / 20) to measure wh
 
 Prints one JSON line: audio-s/s of the queue and of the static batches, their ratio, the ideal ratio sum(max of each static batch) /
 sum(lengths) * B ... and the GPU's name, power limit and clocks.
+
+With `--voices K` every request also carries voice samples, as a service with a fixed voice library sees them: K speaker combinations of
+1-4 speakers with 10-30 s synthetic wavs each, given to the requests in round robin, the voice section in front of the --prompt script
+tokens.  Then only the queue is measured: each request's voices are encoded and prefilled at admission, or, with `--presets`, each
+combination is a `VoicePreset` made once before the passes and the requests attach its shared KV pages (every pass starts a new queue,
+so each pass prefills each preset once).  The JSON line adds the time the queue spent admitting (CUDA events around admission and
+prompt prefill, per pass) and the KV pages the pool held after each frame (peak and mean).
+
+    python tools/bench_queue.py --preset 1.5b --batch 8 --requests 48 --voices 6 [--presets]
 """
 import argparse
 import json
@@ -55,7 +64,11 @@ def main():
     ap.add_argument("--frames", default="8,96,16,64,24,128,12,48,32,80,20,40", help="speech frames per request (cycled)")
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--voices", type=int, default=0, help="voice library size K (0: requests without voices)")
+    ap.add_argument("--presets", action="store_true", help="with --voices: serve the library as voice presets")
     args = ap.parse_args()
+    if args.presets and not args.voices:
+        sys.exit("--presets needs --voices K")
     if not torch.cuda.is_available():
         sys.exit("bench_queue.py measures the GPU: no CUDA device")
     from vibevoice_b200.configuration import preset_config
@@ -68,7 +81,7 @@ def main():
     tok = SynthTokenizer(cfg.decoder_config.vocab_size)
     B = args.batch
     model = VibeVoiceForConditionalGenerationInference(cfg, tok, max_batch=B, prefill_impl="native")
-    parts = ("lm", "head", "acoustic_decoder", "semantic", "connectors", "lm_head")
+    parts = ("lm", "head", "acoustic_decoder", "semantic", "connectors", "lm_head") + (("acoustic_encoder",) if args.voices else ())
     model.load_state_dict(iter_synth_state_dict_fast(cfg, 1234, device=dev, parts=parts), tok)
     eng = model.engine
     d, eos = tok.speech_diffusion_id, tok.eos_token_id
@@ -117,6 +130,9 @@ def main():
             del eng.read_tokens
         return sum(o.speech_outputs[0].shape[-1] for _, o in outs if o.speech_outputs[0] is not None) / SR
 
+    if args.voices:
+        voice_queue(args, model, tok, eng, prompts, frames, audio_s, max_new, timed)
+        return
     res = {}
     for name, fn in [("static", static_pass), ("queue", lambda: queue_pass(lambda i: args.steps)),
                      ("queue_mixed_steps", lambda: queue_pass(lambda i: [5, 10, 20][i % 3]))]:
@@ -134,6 +150,102 @@ def main():
                           queue_mixed_steps_5_10_20=res["queue_mixed_steps"],
                           queue_over_static=res["queue"]["audio_s_per_s"] / res["static"]["audio_s_per_s"],
                           static_padding_bound=bound, gpu=gpu_info())))
+
+
+def voice_library(k, cfg, tok, seed=0):
+    """k voice prompt prefixes (system prompt ids + " Speaker s:" <speech_start> <speech_diffusion> x frames <speech_end> per speaker) in
+    `VibeVoiceProcessor.voice_prefix`'s format: combination j has 1 + j % 4 speakers of 10-30 s of synthetic audio."""
+    g = torch.Generator().manual_seed(seed)
+    V = min(cfg.decoder_config.vocab_size, 151643)
+    rnd = lambda n: torch.randint(0, V, (n,), generator=g).tolist()
+    lib = []
+    for j in range(k):
+        secs = [10 + (7 * j + 11 * s) % 21 for s in range(1 + j % 4)]
+        wavs = torch.zeros(len(secs), max(secs) * SR)
+        ids, sim = rnd(30), [False] * 30
+        for s, sec in enumerate(secs):
+            wavs[s, :sec * SR] = torch.randn(sec * SR, generator=g) * 0.1
+            n = -(-sec * SR // HOP)                  # ceil, as the processor counts a voice's frames
+            ids += rnd(4) + [tok.speech_start_id] + [tok.speech_diffusion_id] * n + [tok.speech_end_id] + rnd(1)
+            sim += [False] * 5 + [True] * n + [False] * 2
+        masks = torch.zeros(len(secs), -(-max(secs) * SR // HOP), dtype=torch.bool)
+        for s, sec in enumerate(secs):
+            masks[s, :-(-sec * SR // HOP)] = True
+        lib.append(dict(input_ids=torch.tensor([ids]), speech_input_mask=torch.tensor([sim]), speech_tensors=wavs, speech_masks=masks))
+    return lib
+
+
+def voice_queue(args, model, tok, eng, prompts, frames, audio_s, max_new, timed):
+    from vibevoice_b200.serving import RequestQueue
+    lib = voice_library(args.voices, model.config, tok)
+    presets = [model.voice_preset(p, seed=j) for j, p in enumerate(lib)] if args.presets else None
+    reqs = []
+    for i, pr in enumerate(prompts):
+        j = i % args.voices
+        ids = torch.cat([lib[j]["input_ids"], pr], dim=1)
+        sim = torch.cat([lib[j]["speech_input_mask"], torch.zeros_like(pr, dtype=torch.bool)], dim=1)
+        reqs.append((dict(input_ids=ids, speech_input_mask=sim, speech_tensors=lib[j]["speech_tensors"], speech_masks=lib[j]["speech_masks"]),
+                     None if presets is None else presets[j]))
+    Lmax = max(r["input_ids"].shape[1] for r, _ in reqs)
+    d, eos = tok.speech_diffusion_id, tok.eos_token_id
+    B = args.batch
+    stats = {}
+
+    def queue_pass():
+        q = RequestQueue(model, max_total_tokens=B * (Lmax + max_new + 8) + B * (max_new + 8))
+        for i, (inp, p) in enumerate(reqs):
+            q.submit(inp, cfg_scale=1.3, steps=args.steps, max_new_tokens=max_new, max_length_times=1e9, seed=i, voice_preset=p)
+        read, admit, prefill, frame = eng.read_tokens, q._admit, q._prefill_progress, q._frame
+        ev, pages = [], []
+
+        def on_events(fn):                    # admission and prompt prefill between two CUDA events on the engine stream
+            def run(*a):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(eng.stream)
+                out = fn(*a)
+                e1.record(eng.stream)
+                ev.append((e0, e1))
+                return out
+            return run
+
+        def scripted():
+            t, lg = read()
+            t = t.copy()
+            for r, row in enumerate(q._rows):
+                if row is not None and row.step >= 0:
+                    t[r] = d if row.step < frames[row.req.rid] else eos
+            return t, lg
+
+        def framed():
+            out = frame()
+            pages.append(eng.kv_pages - eng.kv_pages_free())
+            return out
+        eng.read_tokens, q._admit, q._prefill_progress, q._frame = scripted, on_events(admit), on_events(prefill), framed
+        try:
+            outs = list(q.run())
+        finally:
+            del eng.read_tokens
+        eng.sync()
+        stats["admit_ms"] = sum(a.elapsed_time(b) for a, b in ev)
+        stats["pages_peak"], stats["pages_mean"] = max(pages), sum(pages) / len(pages)
+        return sum(o.speech_outputs[0].shape[-1] for _, o in outs if o.speech_outputs[0] is not None) / SR
+
+    queue_pass()                              # warm-up: programs built, graphs captured
+    ms, admit, peak, mean = [], [], [], []
+    for _ in range(args.runs):
+        t, out_s = timed(eng, queue_pass)
+        assert abs(out_s - audio_s) < 1e-6, (out_s, audio_s)
+        ms.append(t)
+        admit.append(stats["admit_ms"])
+        peak.append(stats["pages_peak"])
+        mean.append(stats["pages_mean"])
+    print(json.dumps(dict(tool="bench_queue", preset=args.preset, batch=B, requests=args.requests, prompt_tokens=args.prompt, frames=frames,
+                          steps=args.steps, audio_s=audio_s, voices=args.voices, presets=bool(args.presets),
+                          voice_prefix_tokens=[int(p["input_ids"].shape[1]) for p in lib],
+                          queue=dict(ms_median=statistics.median(ms), ms_all=[round(x, 1) for x in ms],
+                                     audio_s_per_s=audio_s / (statistics.median(ms) / 1e3)),
+                          admit_ms_median=statistics.median(admit), admit_ms_all=[round(x, 1) for x in admit],
+                          kv_pages_peak=max(peak), kv_pages_mean=statistics.median(mean), kv_pages_total=eng.kv_pages, gpu=gpu_info())))
 
 
 if __name__ == "__main__":

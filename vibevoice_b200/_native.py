@@ -55,6 +55,11 @@ SYMBOLS = {
     "vv_kv_delete_slot": (_I, [_P, _I, _L, _P]),
     "vv_kv_pages_free": (_L, [_P]),
     "vv_kv_pages_total": (_L, [_P]),
+    "vv_kv_prefix_create": (_I, [_P, _I, _L, C.POINTER(C.c_int)]),
+    "vv_kv_prefix_attach": (_I, [_P, _I, _I, _P]),
+    "vv_kv_prefix_release": (_I, [_P, _I]),
+    "vv_kv_prefix_tokens": (_L, [_P, _I]),
+    "vv_kv_seq_pages": (_L, [_P, _I]),
     "vv_set_rope_inv_freq": (_I, [_P, _P, _I]),
     "vv_set_row_mode": (_I, [_P, _P, _P]),
     "vv_lm_decode": (_I, [_P, _P, _P, _P, _P, _P]),

@@ -134,6 +134,9 @@ struct vv_ctx {
   int64_t n_pages = 0; int max_pages = 0; bf16 *kpool = nullptr, *vpool = nullptr;
   int* page_table_dev = nullptr; int* kv_len_dev = nullptr; int* row_mode_dev = nullptr;
   std::vector<int64_t> kv_len_host; std::vector<std::vector<int>> seq_pages; std::vector<int> free_pages;
+  // shared prefixes: page_ref[p] = sequences + prefixes holding page p; shared_len[seq] = positions of seq in shared (immutable) pages
+  struct Prefix { std::vector<int> pages; int64_t n_tokens; };
+  std::vector<int> page_ref; std::vector<int64_t> shared_len; std::map<int, Prefix> prefixes; int next_prefix = 1;
   // scratch
   float* s_lgu = nullptr;   // LM gate/up raw sums [2B][2I] (weight-stream path)
   float *s_h = nullptr, *s_qkv = nullptr;
@@ -1227,6 +1230,7 @@ extern "C" int vv_finalize_weights(vv_ctx* c) {
   }
   c->kv_len_host.assign(M2, 0);
   c->seq_pages.assign(M2, {});
+  c->shared_len.assign(M2, 0);
   for (auto& r : c->raw) if (r.second.p) { cudaFree(r.second.p); r.second.p = nullptr; }
   CK(cudaDeviceSynchronize());
   c->finalized = true;
@@ -1300,7 +1304,9 @@ extern "C" int vv_kv_init(vv_ctx* c, int64_t n_pages) {
       else ++it;
     }
     std::fill(c->kv_len_host.begin(), c->kv_len_host.end(), 0);
+    std::fill(c->shared_len.begin(), c->shared_len.end(), 0);
     for (auto& pg : c->seq_pages) pg.clear();
+    c->prefixes.clear();                  // handles are never reused (next_prefix keeps counting), so old ones stay invalid
   }
   const auto& d = c->d;
   const size_t per_layer = (size_t)n_pages * d.num_kv_heads * KV_PAGE * d.head_dim;
@@ -1312,6 +1318,7 @@ extern "C" int vv_kv_init(vv_ctx* c, int64_t n_pages) {
   RET(dmalloc(c, &c->page_table_dev, nt));
   c->free_pages.clear();
   for (int i = (int)n_pages - 1; i >= 0; --i) c->free_pages.push_back(i);
+  c->page_ref.assign(n_pages, 0);
   return 0;
 }
 extern "C" int64_t vv_kv_pages_free(vv_ctx* c) { return c ? (int64_t)c->free_pages.size() : -1; }
@@ -1324,12 +1331,33 @@ struct PageVals { int v[32]; };
 // block (i, layer) zeroes the K and V rows of page pv.v[i] in that layer; block (0, 0) also writes the page-table entries.  A page handed out
 // again can hold a previous owner's entries, non-finite ones included, in the slots past the new owner's length: attention masks their
 // scores, but its P V product would still take 0 * NaN = NaN from them.  Zeroing here, once per page grant, keeps that off the decode step.
-__global__ void page_grant_kernel(int* dst, PageVals pv, int n, bf16* kpool, bf16* vpool, size_t per_layer, size_t page_elems) {
+// zero == 0 writes the entries only: an attached shared prefix keeps its pages' contents.
+__global__ void page_grant_kernel(int* dst, PageVals pv, int n, int zero, bf16* kpool, bf16* vpool, size_t per_layer, size_t page_elems) {
   if (blockIdx.x == 0 && blockIdx.y == 0 && (int)threadIdx.x < n) dst[threadIdx.x] = pv.v[threadIdx.x];
+  if (!zero) return;
   const size_t o = per_layer * blockIdx.y + (size_t)pv.v[blockIdx.x] * page_elems;
   uint4* k = reinterpret_cast<uint4*>(kpool + o);
   uint4* v = reinterpret_cast<uint4*>(vpool + o);
   for (size_t i = threadIdx.x; i < page_elems / 8; i += blockDim.x) { k[i] = make_uint4(0u, 0u, 0u, 0u); v[i] = make_uint4(0u, 0u, 0u, 0u); }
+}
+
+// page-table entries [first, end) of seq from seq_pages, 32 per launch; zero: the pages are new to seq and get K = V = 0
+static int write_page_entries(vv_ctx* c, int seq, size_t first, bool zero, cudaStream_t s) {
+  const auto& pg = c->seq_pages[seq];
+  const auto& d = c->d;
+  const size_t page_elems = (size_t)d.num_kv_heads * KV_PAGE * d.head_dim;
+  while (first < pg.size()) {
+    PageVals pv;
+    const int n = (int)std::min<size_t>(32, pg.size() - first);
+    for (int i = 0; i < 32; ++i) pv.v[i] = i < n ? pg[first + i] : 0;
+    page_grant_kernel<<<zero ? dim3(n, d.num_layers) : dim3(1, 1), 256, 0, s>>>(c->page_table_dev + (size_t)seq * c->max_pages + first, pv, n,
+                                                                               zero ? 1 : 0, c->kpool, c->vpool, (size_t)c->n_pages * page_elems,
+                                                                               page_elems);
+    CKL();
+    c->launches++;
+    first += n;
+  }
+  return 0;
 }
 
 extern "C" int vv_kv_reserve(vv_ctx* c, int seq, int64_t n_tokens, void* stream) {
@@ -1343,26 +1371,20 @@ extern "C" int vv_kv_reserve(vv_ctx* c, int seq, int64_t n_tokens, void* stream)
     if (c->free_pages.empty()) return fail(VV_ERR_NOMEM, "KV page pool exhausted (seq %d needs %lld pages)", seq, (long long)needp);
     pg.push_back(c->free_pages.back());
     c->free_pages.pop_back();
+    c->page_ref[pg.back()] = 1;
   }
-  while (first < pg.size()) {
-    PageVals pv;
-    const int n = (int)std::min<size_t>(32, pg.size() - first);
-    for (int i = 0; i < 32; ++i) pv.v[i] = i < n ? pg[first + i] : 0;
-    const auto& d = c->d;
-    const size_t page_elems = (size_t)d.num_kv_heads * KV_PAGE * d.head_dim;
-    page_grant_kernel<<<dim3(n, d.num_layers), 256, 0, (cudaStream_t)stream>>>(c->page_table_dev + (size_t)seq * c->max_pages + first, pv, n,
-                                                                                 c->kpool, c->vpool, (size_t)c->n_pages * page_elems, page_elems);
-    CKL();
-    c->launches++;
-    first += n;
-  }
-  return 0;
+  return write_page_entries(c, seq, first, true, (cudaStream_t)stream);
 }
-// pages beyond the new length go back to the free list (a negative stream restarts at every <speech_start>; a server reuses rows)
+// drop one reference to page p: it returns to the free list when nothing holds it any more
+static void unref_page(vv_ctx* c, int p) {
+  if (--c->page_ref[p] == 0) c->free_pages.push_back(p);
+}
+// pages beyond the new length are let go (a negative stream restarts at every <speech_start>; a server reuses rows)
 static void release_pages(vv_ctx* c, int seq, int64_t len) {
   auto& pg = c->seq_pages[seq];
   const size_t keep = (size_t)((len + KV_PAGE - 1) / KV_PAGE);
-  while (pg.size() > keep) { c->free_pages.push_back(pg.back()); pg.pop_back(); }
+  while (pg.size() > keep) { unref_page(c, pg.back()); pg.pop_back(); }
+  if (len == 0) c->shared_len[seq] = 0;
 }
 
 struct Lens { int v[MAX_SEQ]; };
@@ -1381,6 +1403,9 @@ extern "C" int vv_kv_set_len(vv_ctx* c, int seq, int64_t len, void* stream) {
   if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
   if (seq < 0 || seq >= 2 * c->d.max_batch) return fail(VV_ERR_INVALID, "bad seq %d", seq);
   if (len < 0 || len > (int64_t)c->seq_pages[seq].size() * KV_PAGE) return fail(VV_ERR_INVALID, "vv_kv_set_len: %lld outside the reserved range of seq %d", (long long)len, seq);
+  if (len > 0 && len < c->shared_len[seq])
+    return fail(VV_ERR_INVALID, "vv_kv_set_len: %lld would cut into the %lld shared positions of seq %d (0 drops them)", (long long)len,
+                (long long)c->shared_len[seq], seq);
   c->kv_len_host[seq] = len;
   release_pages(c, seq, len);
   return push_lens(c, (cudaStream_t)stream);
@@ -1409,6 +1434,9 @@ extern "C" int vv_kv_delete_slot(vv_ctx* c, int seq, int64_t pos, void* stream) 
   if (seq < 0 || seq >= 2 * c->d.max_batch) return fail(VV_ERR_INVALID, "bad seq %d", seq);
   const int64_t len = c->kv_len_host[seq];
   if (pos < 0 || pos >= len) return fail(VV_ERR_INVALID, "vv_kv_delete_slot: position %lld outside [0,%lld)", (long long)pos, (long long)len);
+  if (pos < c->shared_len[seq])
+    return fail(VV_ERR_INVALID, "vv_kv_delete_slot: position %lld lies in the %lld shared positions of seq %d", (long long)pos,
+                (long long)c->shared_len[seq], seq);
   const auto& d = c->d;
   if (pos != len - 1) {
     const size_t per_layer = (size_t)c->n_pages * d.num_kv_heads * KV_PAGE * d.head_dim;
@@ -1438,6 +1466,10 @@ extern "C" int vv_set_rope_inv_freq(vv_ctx* c, const float* f, int n) {
 }
 extern "C" int vv_kv_write(vv_ctx* c, int seq, int layer, int64_t pos0, int64_t n_tokens, const void* k, const void* v, void* stream) {
   if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  if (seq < 0 || seq >= 2 * c->d.max_batch) return fail(VV_ERR_INVALID, "bad seq %d", seq);
+  if (pos0 < c->shared_len[seq])
+    return fail(VV_ERR_INVALID, "vv_kv_write: position %lld lies in the %lld shared positions of seq %d", (long long)pos0,
+                (long long)c->shared_len[seq], seq);
   RET(vv_kv_reserve(c, seq, pos0 + n_tokens, stream));
   const auto& d = c->d;
   const size_t per_layer = (size_t)c->n_pages * d.num_kv_heads * KV_PAGE * d.head_dim;
@@ -1447,6 +1479,59 @@ extern "C" int vv_kv_write(vv_ctx* c, int seq, int layer, int64_t pos0, int64_t 
   CKL();
   c->launches++;
   return 0;
+}
+
+// ---- shared prefixes: whole pages of one sequence, referenced by a handle and attached to others without a copy.  Positions in shared
+// pages are immutable for every holder (the writers above refuse them), so a sequence's next entry always lands in a page of its own.
+extern "C" int vv_kv_prefix_create(vv_ctx* c, int seq, int64_t n_tokens, int* handle) {
+  if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  if (seq < 0 || seq >= 2 * c->d.max_batch || !handle) return fail(VV_ERR_INVALID, "vv_kv_prefix_create: bad seq %d / null handle", seq);
+  if (n_tokens < KV_PAGE || n_tokens % KV_PAGE || n_tokens > c->kv_len_host[seq])
+    return fail(VV_ERR_INVALID, "vv_kv_prefix_create: %lld tokens: a positive multiple of %d at most kv_len %lld of seq %d", (long long)n_tokens,
+                KV_PAGE, (long long)c->kv_len_host[seq], seq);
+  vv_ctx::Prefix p;
+  p.n_tokens = n_tokens;
+  p.pages.assign(c->seq_pages[seq].begin(), c->seq_pages[seq].begin() + n_tokens / KV_PAGE);
+  for (int pg : p.pages) c->page_ref[pg]++;
+  c->shared_len[seq] = std::max(c->shared_len[seq], n_tokens);
+  *handle = c->next_prefix++;
+  c->prefixes.emplace(*handle, std::move(p));
+  return 0;
+}
+
+extern "C" int vv_kv_prefix_attach(vv_ctx* c, int handle, int seq, void* stream) {
+  if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  auto it = c->prefixes.find(handle);
+  if (it == c->prefixes.end()) return fail(VV_ERR_INVALID, "vv_kv_prefix_attach: no prefix %d (released, or dropped by vv_kv_init)", handle);
+  if (seq < 0 || seq >= 2 * c->d.max_batch) return fail(VV_ERR_INVALID, "bad seq %d", seq);
+  if (c->kv_len_host[seq] != 0) return fail(VV_ERR_INVALID, "vv_kv_prefix_attach: seq %d holds %lld entries", seq, (long long)c->kv_len_host[seq]);
+  release_pages(c, seq, 0);               // the page a decode step keeps for the next entry
+  const auto& p = it->second;
+  c->seq_pages[seq] = p.pages;
+  for (int pg : p.pages) c->page_ref[pg]++;
+  RET(write_page_entries(c, seq, 0, false, (cudaStream_t)stream));
+  c->kv_len_host[seq] = c->shared_len[seq] = p.n_tokens;
+  return push_lens(c, (cudaStream_t)stream);
+}
+
+extern "C" int vv_kv_prefix_release(vv_ctx* c, int handle) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  auto it = c->prefixes.find(handle);
+  if (it == c->prefixes.end()) return fail(VV_ERR_INVALID, "vv_kv_prefix_release: no prefix %d", handle);
+  for (int pg : it->second.pages) unref_page(c, pg);
+  c->prefixes.erase(it);
+  return 0;
+}
+
+// a query: an unknown handle returns -1 without touching the last-error message
+extern "C" int64_t vv_kv_prefix_tokens(vv_ctx* c, int handle) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  auto it = c->prefixes.find(handle);
+  return it == c->prefixes.end() ? -1 : it->second.n_tokens;
+}
+extern "C" int64_t vv_kv_seq_pages(vv_ctx* c, int seq) {
+  if (!c || !c->kpool || seq < 0 || seq >= 2 * c->d.max_batch) return -1;
+  return (int64_t)c->seq_pages[seq].size();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2653,6 +2738,9 @@ static int pf_begin(vv_ctx* c, const char* who, int seq, int64_t pos0, int64_t n
   if (seq < 0 || seq >= 2 * d.max_batch) return fail(VV_ERR_INVALID, "%s: bad seq %d", who, seq);
   if (pos0 < 0 || pos0 + n > d.max_position_embeddings)
     return fail(VV_ERR_INVALID, "%s: positions [%lld, %lld) outside [0, %d)", who, (long long)pos0, (long long)(pos0 + n), d.max_position_embeddings);
+  if (pos0 < c->shared_len[seq])
+    return fail(VV_ERR_INVALID, "%s: position %lld lies in the %lld shared positions of seq %d", who, (long long)pos0,
+                (long long)c->shared_len[seq], seq);
   {
     const int64_t needp = (pos0 + n + KV_PAGE - 1) / KV_PAGE, have = (int64_t)c->seq_pages[seq].size();
     if (needp > c->max_pages || needp - have > (int64_t)c->free_pages.size())

@@ -72,6 +72,8 @@ class Engine:
         self.h = h
         self.finalized = False
         self.kv_pages = 0
+        self.kv_epoch = 0                         # kv_init count: a prefix made in an earlier pool is gone
+        self.prefix_pages: Dict[int, int] = {}
         self.stream = torch.cuda.Stream(device=self.device)
         H, B = config.decoder_config.hidden_size, max_batch
         dev = self.device
@@ -367,6 +369,30 @@ class Engine:
         pages = (total_tokens + 63) // 64 + 2 * self.B * 2
         N.check(self.lib.vv_kv_init(self.h, pages), "vv_kv_init")
         self.kv_pages = pages
+        self.kv_epoch += 1
+        self.prefix_pages = {}                                     # live prefix handle -> its pages
+
+    # shared prefixes (include/vibevoice_b200.h: vv_kv_prefix_*)
+    def kv_prefix_create(self, seq: int, n_tokens: int) -> int:
+        h = C.c_int(0)
+        N.check(self.lib.vv_kv_prefix_create(self.h, int(seq), int(n_tokens), C.byref(h)), "vv_kv_prefix_create")
+        self.prefix_pages[h.value] = int(n_tokens) // 64
+        return h.value
+
+    def kv_prefix_attach(self, handle: int, seq: int):
+        N.check(self.lib.vv_kv_prefix_attach(self.h, int(handle), int(seq), self.s), "vv_kv_prefix_attach")
+
+    def kv_prefix_release(self, handle: int):
+        N.check(self.lib.vv_kv_prefix_release(self.h, int(handle)), "vv_kv_prefix_release")
+        self.prefix_pages.pop(int(handle), None)
+
+    def kv_prefix_tokens(self, handle: int) -> int:
+        """tokens of a live prefix, -1 when the handle is not (released, or dropped by kv_init)."""
+        return int(self.lib.vv_kv_prefix_tokens(self.h, int(handle)))
+
+    def kv_seq_pages(self, seq: int) -> int:
+        """pages sequence `seq` holds, shared ones included (`vv_kv_seq_pages`)."""
+        return int(self.lib.vv_kv_seq_pages(self.h, int(seq)))
 
     def kv_len(self, seq: int) -> int:
         return int(self.lib.vv_kv_len(self.h, seq))

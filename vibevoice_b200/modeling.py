@@ -38,6 +38,48 @@ class VibeVoiceGenerationOutput:
     reach_max_step_sample: Optional[torch.BoolTensor] = None
 
 
+class VoicePreset:
+    """A voice prompt prefix (`system prompt + " Voice input:\\n" + speakers`) encoded once by `model.voice_preset()`.
+
+    Holds the prefix ids [Lp], its embeddings [Lp, H] fp32 on the device (token rows with the connected voice frames in place), the voice
+    noise it drew (`noise`, the `_voice_noise` a full-prompt `generate()` takes to reproduce it) and `shared = 64 * (Lp // 64)`: the
+    positions whose K/V live in shared pages of the KV pool.  The first request that uses the preset after a pool (re)initialisation
+    prefills them into its own sequence and makes them a prefix (`vv_kv_prefix_create`); later requests attach that prefix and prefill
+    only from `shared` on.  `release()` gives the pages back; the next use builds them again."""
+
+    def __init__(self, model, ids: torch.Tensor, embeds: torch.Tensor, noise):
+        self.model, self.ids, self.embeds, self.noise = model, ids, embeds, noise
+        self.shared = ids.numel() // 64 * 64
+        self._eng, self._epoch, self._handle = None, -1, None
+
+    @property
+    def pages(self) -> int:
+        return self.shared // 64
+
+    def resident(self) -> bool:
+        """whether the shared pages are in the model's current KV pool."""
+        eng = self.model.engine
+        return (self._handle is not None and eng is self._eng and eng.kv_epoch == self._epoch
+                and eng.kv_prefix_tokens(self._handle) == self.shared)
+
+    def _attach(self, seq: int) -> bool:
+        if not self.resident():
+            return False
+        self._eng.kv_prefix_attach(self._handle, seq)
+        return True
+
+    def _adopt(self, seq: int):
+        """the first `shared` positions of `seq` (prefilled from `embeds`) become the preset's pages."""
+        eng = self.model.engine
+        self._handle, self._eng, self._epoch = eng.kv_prefix_create(seq, self.shared), eng, eng.kv_epoch
+
+    def release(self):
+        """Give the shared pages back to the pool (sequences attached to them keep them until they are reset)."""
+        if self.resident():
+            self._eng.kv_prefix_release(self._handle)
+        self._handle = self._eng = None
+
+
 class ForcedTokenScript:
     """Accepted as (an element of) `logits_processor`: per-row token scripts that override the constrained argmax,
     e.g. "speech_diffusion x F then EOS" (BASELINE.md section 3).  The reference achieves the same with a
@@ -241,18 +283,86 @@ class VibeVoiceForConditionalGenerationInference:
         tc, dev = self.config.acoustic_tokenizer_config, eng.device
         wavs = torch.as_tensor(speech_tensors)
         n, T = wavs.shape
-        shape = (n, eng.voice_frames(T), self.config.acoustic_vae_dim)
+        std_n, eps = self._draw_voice_noise(n, T, generator) if noise is None else noise
         if tc.std_dist_type == "gaussian":
-            std_n = torch.randn(n, device=dev, generator=generator) if noise is None else noise[0].to(dev, torch.float32)
-            eps = torch.randn(shape, device=dev, generator=generator) if noise is None else noise[1].to(dev, torch.float32)
-            sigma = std_n * (float(tc.fix_std) / 0.8)
+            sigma = std_n.to(dev, torch.float32) * (float(tc.fix_std) / 0.8)
+            eps = eps.to(dev, torch.float32)
         elif tc.std_dist_type == "fix":
-            eps = torch.randn(shape, device=dev, generator=generator) if noise is None else noise[1].to(dev, torch.float32)
+            eps = eps.to(dev, torch.float32)
             sigma = torch.full((n,), float(tc.fix_std), device=dev)
         else:
             eps, sigma = None, torch.zeros(n, device=dev)
         emb = eng.voice_encode(wavs, sigma, eps)
         return emb[torch.as_tensor(speech_masks).to(dev).bool()]
+
+    def _draw_voice_noise(self, n: int, T: int, generator: Optional[torch.Generator] = None):
+        """(std_n [n], eps [n, F, vae_dim]) of `_voice_prompt` for n voices of T samples, in PyTorch's sampling order; a part the
+        checkpoint's std_dist_type does not use is None and is not drawn."""
+        tc, eng = self.config.acoustic_tokenizer_config, self.engine
+        shape = (n, eng.voice_frames(T), self.config.acoustic_vae_dim)
+        std_n = torch.randn(n, device=eng.device, generator=generator) if tc.std_dist_type == "gaussian" else None
+        eps = torch.randn(shape, device=eng.device, generator=generator) if tc.std_dist_type in ("gaussian", "fix") else None
+        return std_n, eps
+
+    @torch.no_grad()
+    def voice_preset(self, prefix_inputs, seed: Optional[int] = None, generator: Optional[torch.Generator] = None) -> "VoicePreset":
+        """Encode a voice prompt prefix once (`VibeVoiceProcessor.voice_prefix`: ids, speech_input_mask, speech_tensors, speech_masks)
+        for `generate(..., voice_preset=)` and `RequestQueue.submit(..., voice_preset=)`.  The voice noise comes from `generator` (a
+        device generator), else a device generator seeded with `seed`, else the device RNG, and is kept (`VoicePreset.noise`), so a
+        preset made with the same seed is the same.  The prefix's K/V is prefilled by the first request that uses it."""
+        eng = self.engine
+        if eng is None or not eng.finalized:
+            raise N.VVError("weights not loaded")
+        if self._voice is None:
+            raise N.VVError("voice presets need the acoustic tokenizer encoder weights, which this checkpoint does not have")
+        ids = torch.as_tensor(prefix_inputs["input_ids"]).cpu().long()
+        sim = torch.as_tensor(prefix_inputs["speech_input_mask"]).cpu().bool()
+        if ids.dim() == 2 and ids.shape[0] != 1 or sim.shape != ids.shape:
+            raise ValueError("voice_preset: one prefix (input_ids %s, speech_input_mask %s)" % (tuple(ids.shape), tuple(sim.shape)))
+        ids, sim = ids.reshape(-1), sim.reshape(-1)
+        wavs, masks = torch.as_tensor(prefix_inputs["speech_tensors"]), torch.as_tensor(prefix_inputs["speech_masks"]).bool()
+        if int(masks.sum()) != int(sim.sum()):
+            raise ValueError("voice_preset: %d speech positions for %d voice frames" % (int(sim.sum()), int(masks.sum())))
+        if generator is None and seed is not None:
+            generator = torch.Generator(device=eng.device).manual_seed(int(seed))
+        with torch.cuda.stream(eng.stream):
+            noise = self._draw_voice_noise(wavs.shape[0], wavs.shape[1], generator)
+            ve = self._voice(wavs, masks, self._scale, self._bias, noise=noise)
+            e = eng.embed_gather(ids).clone()
+            e[sim.to(e.device)] = ve.to(e.device, e.dtype)
+        return VoicePreset(self, ids, e, noise)
+
+    def _presets_of(self, voice_preset, b: int) -> List[Optional["VoicePreset"]]:
+        ps = list(voice_preset) if isinstance(voice_preset, (list, tuple)) else [voice_preset] * b
+        if len(ps) != b:
+            raise ValueError("voice_preset: %d presets for %d rows" % (len(ps), b))
+        for p in ps:
+            if p is not None and (not isinstance(p, VoicePreset) or p.model is not self):
+                raise ValueError("voice_preset: a preset made by model.voice_preset() of this model (or None)")
+        return ps
+
+    @staticmethod
+    def _check_preset_row(p: "VoicePreset", ids: torch.Tensor, sim: Optional[torch.Tensor], what: str):
+        """ids / sim: one row's unpadded prompt ids and speech mask (sim may be None)."""
+        Lp = p.ids.numel()
+        if ids.numel() <= Lp or not torch.equal(ids[:Lp], p.ids):
+            raise ValueError("voice_preset: %s does not start with the preset's %d prefix ids (followed by the script)" % (what, Lp))
+        if sim is not None and bool(sim[Lp:].any()):
+            raise ValueError("voice_preset: %s has speech positions past the preset's prefix" % what)
+
+    def _preset_embeds(self, p: "VoicePreset", ids: torch.Tensor) -> torch.Tensor:
+        """[L, H] prompt embeddings of a row whose unpadded ids start with the preset's: its embeddings, then the rest gathered."""
+        return torch.cat([p.embeds, self.engine.embed_gather(ids[p.ids.numel():])])
+
+    def _preset_prefill(self, p: "VoicePreset", seq: int, embeds: torch.Tensor) -> torch.Tensor:
+        """Native prefill of an empty sequence whose prompt starts with the preset: attach the shared pages, or prefill them and make
+        them the preset's; then the rest from position `shared`.  -> final-norm hidden of the last row.  The caller sets the length."""
+        eng = self.engine
+        if p.shared and not p._attach(seq):
+            eng.lm_prefill(seq, embeds[:p.shared])
+            eng.kv_set_len(seq, p.shared)
+            p._adopt(seq)
+        return eng.lm_prefill(seq, embeds[p.shared:], pos0=p.shared)
 
     @classmethod
     def from_pretrained(cls, path: str, torch_dtype=None, device_map=None, attn_implementation=None, tokenizer=None,
@@ -374,14 +484,16 @@ class VibeVoiceForConditionalGenerationInference:
     def _reserve_kv(self, total_tokens: int):
         eng = self.engine
         need_pages = (total_tokens + 63) // 64 + 4 * eng.B          # every sequence may hold one partially filled page
-        if eng.kv_pages < need_pages:
+        held = sum((getattr(eng, "prefix_pages", None) or {}).values())     # voice presets' shared pages stay in the pool
+        if eng.kv_pages - held < need_pages:
             eng.kv_init(total_tokens)                                # first call, or a later call that needs more: the pool is re-sized
 
     def _prefill_rows(self, b, input_ids, attention_mask, lens, use_voice, speech_tensors, speech_masks, speech_input_mask, voice_noise,
-                      gather, run) -> List[torch.Tensor]:
+                      gather, run, presets=None) -> List[torch.Tensor]:
         """Whole-prompt prefill of rows 0..b-1, one call per row: `gather(ids)` embeds the unpadded ids, the voice embeddings are scattered
         at `speech_input_mask` (:216-224: acoustic encoder -> sample -> (x+bias)*scale -> connector), `run(r, embeds)` fills the K/V of
-        sequence r and returns its last final-norm hidden state; the row's length is then set.  -> hidden states of the rows."""
+        sequence r and returns its last final-norm hidden state; the row's length is then set.  A row with a voice preset
+        (`presets[r]`) takes the preset's embeddings and shared pages and the native prefill instead.  -> hidden states of the rows."""
         eng = self.engine
         hids = []
         with torch.cuda.stream(eng.stream):
@@ -396,6 +508,11 @@ class VibeVoiceForConditionalGenerationInference:
                     offs.append(offs[-1] + int(c_))
             for r in range(b):
                 keep = attention_mask[r].bool()
+                if presets is not None and presets[r] is not None:
+                    ids_r = input_ids[r][keep]
+                    hids.append(self._preset_prefill(presets[r], r, self._preset_embeds(presets[r], ids_r)))
+                    eng.kv_set_len(r, int(lens[r]))
+                    continue
                 e = gather(input_ids[r][keep])
                 if voice_embeds is not None and counts[r]:
                     e = e.clone()
@@ -409,8 +526,12 @@ class VibeVoiceForConditionalGenerationInference:
                  prefix_allowed_tokens_fn=None, synced_gpus=None, assistant_model=None, audio_streamer=None,
                  negative_prompt_ids=None, negative_prompt_attention_mask=None, speech_tensors=None, speech_masks=None,
                  speech_input_mask=None, is_prefill: bool = True, return_speech: bool = True, cfg_scale: float = 1.0,
-                 stop_check_fn: Optional[Callable[[], bool]] = None, tqdm_class=None, **kwargs) -> VibeVoiceGenerationOutput:
-        """`modeling_vibevoice_inference.py:326-695`."""
+                 stop_check_fn: Optional[Callable[[], bool]] = None, tqdm_class=None, voice_preset=None, **kwargs) -> VibeVoiceGenerationOutput:
+        """`modeling_vibevoice_inference.py:326-695`.
+
+        `voice_preset`: a `VoicePreset` for every row, or a list with a preset or None per row.  A row with a preset must start with the
+        preset's prefix ids and have no speech position after them; it runs no voice encoding (its speech inputs, if given, are not
+        used) and is prefilled natively from the preset's shared pages on.  Rows without a preset carry no voice in such a batch."""
         tokenizer = kwargs.pop("tokenizer", None) or self._tok
         kwargs.pop("parsed_scripts", None); kwargs.pop("all_speakers_list", None)
         max_length_times = kwargs.pop("max_length_times", 2)
@@ -424,7 +545,7 @@ class VibeVoiceForConditionalGenerationInference:
             sample_gen = torch.Generator().manual_seed(torch.initial_seed())
         refresh_negative = bool(kwargs.get("refresh_negative", True))
         use_voice = bool(is_prefill and speech_tensors is not None)
-        if use_voice and self._voice is None:
+        if use_voice and self._voice is None and voice_preset is None:
             raise N.VVError("voice-prompt prefill needs the acoustic tokenizer encoder weights, which this checkpoint does not have")
         forced: Optional[ForcedTokenScript] = None
         user_procs = []
@@ -460,6 +581,22 @@ class VibeVoiceForConditionalGenerationInference:
             # the lm_head rows and the constrained argmax were fixed when the weights were packed (:405-419 resolves them per call)
             raise ValueError("tokenizer special ids %s differ from the ids the engine was built with %s; load the model with this "
                              "tokenizer (from_pretrained(..., tokenizer=tok))" % (self._valid_ids(tok), list(eng.valid_ids)))
+        presets = None
+        if voice_preset is not None:
+            if not is_prefill:
+                raise ValueError("voice_preset needs the whole-prompt prefill (is_prefill=True)")
+            if kwargs.get("prefill_impl") == "decode":
+                raise ValueError("voice_preset: prefill_impl=\"decode\" cannot continue a prompt from shared K/V pages")
+            presets = self._presets_of(voice_preset, b)
+            sim_all = None if speech_input_mask is None else torch.as_tensor(speech_input_mask).bool().cpu()
+            for r in range(b):
+                keep = attention_mask[r].bool()
+                sim_r = None if sim_all is None else sim_all[r][keep]
+                if presets[r] is not None:
+                    self._check_preset_row(presets[r], input_ids[r][keep], sim_r, "row %d" % r)
+                elif sim_r is not None and bool(sim_r.any()):
+                    raise ValueError("voice_preset: row %d has voice samples but no preset; give every voiced row a preset" % r)
+            use_voice = False
 
         if kwargs.get("max_new_tokens", None) is None:
             kwargs["max_new_tokens"] = dc.max_position_embeddings - L0                      # :372-373
@@ -489,6 +626,8 @@ class VibeVoiceForConditionalGenerationInference:
         impl = kwargs.get("prefill_impl", self._prefill_impl or "auto")
         use_native_prefill = impl == "native"
         use_torch_prefill = not use_native_prefill and self._prefill is not None and impl != "decode"
+        if presets is not None and not use_torch_prefill:
+            use_native_prefill = True                            # preset rows continue from the pool; the others prefill as usual
         if use_torch_prefill or use_native_prefill:
             # ---- whole-prompt prefill (a-9 / f-2), K/V in the paged pool: library kernels (TorchPrefill) or the engine's (vv_lm_prefill) -----
             if use_torch_prefill:
@@ -497,7 +636,7 @@ class VibeVoiceForConditionalGenerationInference:
             else:
                 gather, run = eng.embed_gather, (lambda r, e: eng.lm_prefill(r, e))
             hids = self._prefill_rows(b, input_ids, attention_mask, lens, use_voice, speech_tensors, speech_masks, speech_input_mask,
-                                      kwargs.get("_voice_noise"), gather, run)
+                                      kwargs.get("_voice_noise"), gather, run, presets)
             eng.embed_tokens([pad_tok] * B + [start_id] * B, eng.embeds)     # negative rows: [<speech_start>] at pos 0 (:379-386)
             eng.lm_decode()
             with torch.cuda.stream(eng.stream):

@@ -218,6 +218,20 @@ class VibeVoiceProcessor:
         mask += [False] * len(t)
         return dict(input_ids=ids, speech_inputs=wavs or None, speech_input_mask=mask, parsed_script=parsed, all_speakers=speakers)
 
+    def voice_prefix(self, voice_samples) -> BatchEncoding:
+        """The prompt prefix `system prompt + " Voice input:\\n" + speakers` of `voice_samples` as tensors: `input_ids` [1, Lp],
+        `speech_input_mask` [1, Lp], `speech_tensors` and `speech_masks` -- exactly the first Lp ids and the speech inputs that
+        `self(text=script, voice_samples=voice_samples)` gives for any script, provided the script has as many speakers as there are
+        voices (the processor keeps the first `len(speakers)` voices).  The input of `model.voice_preset`."""
+        if not voice_samples:
+            raise ValueError("voice_prefix needs at least one voice sample")
+        ids = self._enc(self.system_prompt, special=True)
+        v_ids, wavs, v_mask = self._voice_prompt(voice_samples)
+        sp = self.prepare_speech_inputs(wavs, return_tensors="pt")
+        return BatchEncoding(input_ids=torch.tensor([ids + v_ids], dtype=torch.long),
+                             speech_input_mask=torch.tensor([[False] * len(ids) + v_mask], dtype=torch.bool),
+                             speech_tensors=sp["padded_speeches"], speech_masks=sp["speech_masks"])
+
     def prepare_speech_inputs(self, speech_inputs: List[np.ndarray], return_tensors=None, device=None, dtype=None) -> Dict[str, Any]:
         if not speech_inputs:
             return {"padded_speeches": None, "speech_masks": None}

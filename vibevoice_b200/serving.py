@@ -47,7 +47,8 @@ class _Request:
     max_length: int
     max_steps: int
     max_step_per_sample: int
-    pages: int                          # worst-case KV pages of both sequences
+    pages: int                          # worst-case KV pages of both sequences (with a preset: those outside its shared pages)
+    preset: Any = None                  # VoicePreset or None
 
 
 @dataclass
@@ -58,6 +59,8 @@ class _Row:
     order: int                          # admission order (prefill progress goes oldest first)
     embeds: Optional[torch.Tensor] = None   # prompt embeddings while the prefill runs
     done: int = 0                       # prompt tokens prefilled so far
+    builds: bool = False                # prefilling its preset's shared pages, which become the preset's at `shared`
+    prefix: Optional[int] = None        # handle of the shared pages the row holds (attached or built)
     hid: Optional[torch.Tensor] = None  # final-norm hidden state of the last prompt token
     step: int = -1                      # generation step of the next frame; -1 while admitting
     seq: List[int] = field(default_factory=list)
@@ -94,7 +97,7 @@ class RequestQueue:
         self._waiting: Deque[_Request] = collections.deque()
         self._next_rid = 0
         self._rows: List[Optional[_Row]] = [None] * self.B
-        self._pages_used = 0
+        self._pages_used = 0                               # the live rows' pages (shared prefixes: preset_pages())
         self._admitted = 0
         self._nmax = 0
         self._modes: Optional[List[int]] = None
@@ -102,8 +105,11 @@ class RequestQueue:
     # ---- requests ---------------------------------------------------------------------------------------------------------------------
     def submit(self, inputs, cfg_scale: float = 1.3, steps: int = 10, solver: str = "dpmsolver++", max_new_tokens: Optional[int] = None,
                max_length_times: float = 2, seed: int = 1234, generation_config=None, logits_processor=None, audio_streamer=None,
-               stop_check_fn=None, refresh_negative: bool = True) -> int:
-        """Queue one request; `inputs` is the processor output for ONE script (+ its voices).  Returns the request id `run()` reports."""
+               stop_check_fn=None, refresh_negative: bool = True, voice_preset=None) -> int:
+        """Queue one request; `inputs` is the processor output for ONE script (+ its voices).  Returns the request id `run()` reports.
+        With `voice_preset` (`model.voice_preset`) the prompt must start with the preset's prefix: the request runs no voice encoding,
+        attaches the preset's shared K/V pages (prefilling them first if they are not in the pool) and is prefilled natively from there;
+        its result equals `generate(<that request>, voice_preset=voice_preset)`."""
         if audio_streamer is not None:
             raise ValueError("audio_streamer is not supported by RequestQueue")
         if stop_check_fn is not None:
@@ -136,7 +142,12 @@ class RequestQueue:
         am = torch.ones_like(ids) if am is None else torch.as_tensor(am).cpu().long().reshape(ids.shape)
         st = inputs.get("speech_tensors") if hasattr(inputs, "get") else None
         voice = None
-        if st is not None:
+        if voice_preset is not None:
+            voice_preset = self.model._presets_of(voice_preset, 1)[0]
+            sim = inputs.get("speech_input_mask") if hasattr(inputs, "get") else None
+            sim = None if sim is None else torch.as_tensor(sim).bool().cpu().reshape(ids.shape)[0][am[0].bool()]
+            self.model._check_preset_row(voice_preset, ids[0][am[0].bool()], sim, "the request")
+        elif st is not None:
             if self.model._voice is None:
                 raise N.VVError("voice-prompt prefill needs the acoustic tokenizer encoder weights, which this checkpoint does not have")
             voice = (st, inputs["speech_masks"], torch.as_tensor(inputs["speech_input_mask"]).bool().cpu().reshape(ids.shape)[0])
@@ -149,13 +160,53 @@ class RequestQueue:
         max_steps = min(max_length - L0, int(max_length_times * L0))
         max_step_per_sample = min(max_length - init_len, int(max_length_times * init_len))
         pages = (L0 + max_steps + 2 + 63) // 64 + (max_steps + 2 + 63) // 64
-        if pages > self._budget:
-            raise ValueError("max_total_tokens: the request needs up to %d KV pages, the pool has %d for requests" % (pages, self._budget))
+        shared = 0 if voice_preset is None else voice_preset.pages
+        pages -= shared
+        if pages + shared > self._budget:
+            raise ValueError("max_total_tokens: the request needs up to %d KV pages, the pool has %d for requests" % (pages + shared, self._budget))
         rid = self._next_rid
         self._next_rid += 1
         self._waiting.append(_Request(rid, ids[0], am[0].bool(), voice, float(cfg_scale), steps, solver, int(seed), max_length,
-                                      max_steps, max_step_per_sample, pages))
+                                      max_steps, max_step_per_sample, pages, voice_preset))
         return rid
+
+    def _prefixes(self) -> dict:
+        """handle -> pages of every shared prefix in the pool (this queue's presets, and any other preset used on the model since)."""
+        return getattr(self.eng, "prefix_pages", None) or {}
+
+    def preset_pages(self, extra=None) -> int:
+        """KV pages of shared prefixes: every prefix in the pool, the released ones live rows still hold, and the presets that live rows
+        build or wait for (+ `extra`'s when it is not in the pool)."""
+        held, pending = dict(self._prefixes()), {}
+        for row in self._rows:
+            p = None if row is None else row.req.preset
+            if p is None or not p.shared:
+                continue
+            if row.prefix is not None:
+                held[row.prefix] = p.pages
+            elif not p.resident():
+                pending[id(p)] = p.pages
+        if extra is not None and extra.shared and not extra.resident():
+            pending[id(extra)] = extra.pages
+        return sum(held.values()) + sum(pending.values())
+
+    def _fits(self, req) -> bool:
+        return self._pages_used + self.preset_pages(req.preset) + req.pages <= self._budget
+
+    def _evict(self, req) -> bool:
+        """Release shared prefixes until the request at the head fits: first those no live or waiting request uses, then, with no row
+        live, every one but its own (their requests build them again).  Without the second step a pool filled by resident presets would
+        keep the head waiting for ever; `submit` made sure it fits beside its own preset alone.  Returns whether it fits now."""
+        live = any(row is not None for row in self._rows)
+        keep = {row.prefix for row in self._rows if row is not None}
+        own = {req.preset._handle} if req.preset is not None and req.preset.resident() else set()
+        used = {w.preset._handle for w in self._waiting if w.preset is not None and w.preset.resident()}
+        for spare in ([keep | used | own] if live else [keep | used | own, own]):
+            for h in [h for h in self._prefixes() if h not in spare]:
+                self.eng.kv_prefix_release(h)
+            if self._fits(req):
+                return True
+        return False
 
     # ---- the loop ---------------------------------------------------------------------------------------------------------------------
     def run(self) -> Iterator[Tuple[int, VibeVoiceGenerationOutput]]:
@@ -204,7 +255,7 @@ class RequestQueue:
                                                                 reach_max_step_sample=torch.tensor([False]))))
                 continue
             free = [r for r in range(self.B) if self._rows[r] is None]
-            if not free or self._pages_used + req.pages > self._budget:
+            if not free or not (self._fits(req) or self._evict(req)):
                 break
             self._waiting.popleft()
             self._pages_used += req.pages
@@ -217,7 +268,9 @@ class RequestQueue:
             self._admitted += 1
             with torch.cuda.stream(eng.stream):
                 ids = req.ids[req.keep]
-                if self._native:
+                if req.preset is not None:
+                    e = model._preset_embeds(req.preset, ids)
+                elif self._native:
                     e = eng.embed_gather(ids)
                 else:
                     e = model._lm_sd["model.language_model.embed_tokens.weight"][ids.to(eng.device)]
@@ -236,21 +289,36 @@ class RequestQueue:
         budget = self._chunk
         for r in sorted((r for r in range(B) if self._rows[r] is not None and self._rows[r].step < 0), key=lambda r: self._rows[r].order):
             row = self._rows[r]
+            p = row.req.preset
+            if p is not None and p.shared and row.done == 0 and not row.builds:
+                if p._attach(r):
+                    row.done, row.prefix = p.shared, p._handle
+                elif any(o is not None and o.builds and o.req.preset is p for o in self._rows):
+                    continue                            # attaches once the row building the preset's pages has made them
+                else:
+                    row.builds = True
             n_all = row.embeds.shape[0]
-            n = n_all - row.done
-            if budget is not None:
-                if budget < n:
-                    n = budget // 64 * 64               # chunk boundaries on 64-token rows: the native prefill's own chunk grid
-                budget -= n
+            while True:                                 # a row building its preset stops at `shared` once, to make the prefix
+                n = (p.shared if row.builds else n_all) - row.done
+                if budget is not None:
+                    if budget < n:
+                        n = budget // 64 * 64           # chunk boundaries on 64-token rows: the native prefill's own chunk grid
+                    budget -= n
+                if n <= 0:
+                    break
+                with torch.cuda.stream(eng.stream):
+                    if self._native or p is not None:
+                        row.hid = eng.lm_prefill(r, row.embeds[row.done:row.done + n], pos0=row.done)
+                    else:
+                        row.hid = self.model._prefill.run(eng, r, row.embeds)
+                row.done += n
+                eng.kv_set_len(r, row.done)
+                if not (row.builds and row.done == p.shared):
+                    break
+                p._adopt(r)
+                row.builds, row.prefix = False, p._handle
             if n <= 0:
                 break
-            with torch.cuda.stream(eng.stream):
-                if self._native:
-                    row.hid = eng.lm_prefill(r, row.embeds[row.done:row.done + n], pos0=row.done)
-                else:
-                    row.hid = self.model._prefill.run(eng, r, row.embeds)
-            row.done += n
-            eng.kv_set_len(r, row.done)
             if row.done < n_all:
                 continue
             # step 0 of generate(): the negative sequence restarts at [<speech_start>] (decoded by the next frame's lm_decode, with the
