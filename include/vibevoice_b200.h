@@ -120,6 +120,19 @@ int64_t vv_kv_prefix_tokens(vv_ctx* ctx, int handle);                          /
 int64_t vv_kv_seq_pages(vv_ctx* ctx, int seq);                                 /* pages seq holds, shared ones included; -1 for a bad seq
                                                                                   or before vv_kv_init */
 
+/* ---- parked sequences: a sequence's whole page list set aside and given back later, possibly to another sequence index ------------- *
+ * vv_kv_park moves every page of seq (shared and private, the partly filled last one included) into a parked record with kv_len(seq)
+ * and its shared length; the references move, nothing is copied or launched, and seq is left empty (length 0, no pages).  A sequence of
+ * length 0 is refused.  vv_kv_unpark writes the record's pages into an empty seq's page table (the page it kept for its next entry goes
+ * back first), restores both lengths and invalidates the handle: the next append lands where it would have landed without parking, and
+ * the shared positions stay immutable.  Parked pages count as used in vv_kv_pages_free.  vv_kv_init drops every parked record; handles
+ * are never reused.  Every refusal returns VV_ERR_INVALID / VV_ERR_STATE and launches nothing. */
+int vv_kv_park(vv_ctx* ctx, int seq, int* handle);
+int vv_kv_unpark(vv_ctx* ctx, int handle, int seq, void* stream);
+int vv_kv_park_release(vv_ctx* ctx, int handle);                               /* drop a parked record's references */
+int64_t vv_kv_parked_pages(vv_ctx* ctx, int handle);                           /* pages of a live record, else -1 (a query: no error
+                                                                                  message is recorded) */
+
 /* ---- a-3: LLM decode step for pos+neg rows in ONE weight pass ---------------------------------- *
  * replaces self(**model_inputs) at :480-482 and the negative forward at :583-585.
  * embeds [2B,H] fp32 (row r<B positive, r>=B negative).  Every row with row_mode 1 (default: all)
@@ -190,6 +203,12 @@ int vv_connect(vv_ctx* ctx, const float* latent /*[B,64]*/, const float* sem /*[
                float* embeds_inout /*[2B,H]: rows r<B overwritten where active*/, void* stream);
 int vv_codec_state_zero(vv_ctx* ctx, const int32_t* rows_host, int n, void* stream);   /* <speech_end>, :542-546 */
 int vv_codec_state_reset(vv_ctx* ctx, void* stream);                                    /* new generate() call */
+/* one row's committed streaming state (acoustic decoder, then semantic encoder: what vv_codec_state_zero zeroes) <-> a contiguous fp32
+ * device buffer of vv_codec_state_floats() values, in one launch each, bit for bit: a row loaded with another row's saved state
+ * continues as that row did (to the rounding of the codec's split-K atomics), so a request parked between frames resumes on any row. */
+int64_t vv_codec_state_floats(vv_ctx* ctx);
+int vv_codec_state_save(vv_ctx* ctx, int row, float* out, void* stream);
+int vv_codec_state_load(vv_ctx* ctx, int row, const float* in, void* stream);
 
 /* ---- fused frame tail: sampler -> decoder -> semantic -> connectors in one enqueue ------------- *
  * (:626-672).  Also copies the positive rows' next embeddings into the negative rows of `embeds_inout`

@@ -60,6 +60,10 @@ SYMBOLS = {
     "vv_kv_prefix_release": (_I, [_P, _I]),
     "vv_kv_prefix_tokens": (_L, [_P, _I]),
     "vv_kv_seq_pages": (_L, [_P, _I]),
+    "vv_kv_park": (_I, [_P, _I, C.POINTER(C.c_int)]),
+    "vv_kv_unpark": (_I, [_P, _I, _I, _P]),
+    "vv_kv_park_release": (_I, [_P, _I]),
+    "vv_kv_parked_pages": (_L, [_P, _I]),
     "vv_set_rope_inv_freq": (_I, [_P, _P, _I]),
     "vv_set_row_mode": (_I, [_P, _P, _P]),
     "vv_lm_decode": (_I, [_P, _P, _P, _P, _P, _P]),
@@ -80,6 +84,9 @@ SYMBOLS = {
     "vv_connect": (_I, [_P, _P, _P, _P, _P, _P]),
     "vv_codec_state_zero": (_I, [_P, _P, _I, _P]),
     "vv_codec_state_reset": (_I, [_P, _P]),
+    "vv_codec_state_floats": (_L, [_P]),
+    "vv_codec_state_save": (_I, [_P, _I, _P, _P]),
+    "vv_codec_state_load": (_I, [_P, _I, _P, _P]),
     "vv_frame_tail": (_I, [_P, _P, _P, _P, _F, _P, _P, _P, _P]),
     "vv_voice_encode_workspace": (_L, [_P, _I, _L]),
     "vv_voice_encode": (_I, [_P, _P, _I, _L, _P, _P, _P, _P, _P, _L, _P]),

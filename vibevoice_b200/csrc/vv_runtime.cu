@@ -76,6 +76,7 @@ struct Codec {
   std::vector<int> T;                        // frames per stage (per 1 latent frame)
   std::vector<int> C;
   StateSeg* segs_dev = nullptr; int n_segs = 0;
+  int64_t state_floats = 0;                  // one row's history: the sum of the segments' n
   int64_t weight_bytes = 0;
 };
 struct VoiceEnc {           // non-streaming acoustic encoder for voice prompts (a-9); present iff the checkpoint has its tensors
@@ -137,6 +138,9 @@ struct vv_ctx {
   // shared prefixes: page_ref[p] = sequences + prefixes holding page p; shared_len[seq] = positions of seq in shared (immutable) pages
   struct Prefix { std::vector<int> pages; int64_t n_tokens; };
   std::vector<int> page_ref; std::vector<int64_t> shared_len; std::map<int, Prefix> prefixes; int next_prefix = 1;
+  // parked sequences: a sequence's whole page list with its lengths, holding the references it took (vv_kv_park)
+  struct Parked { std::vector<int> pages; int64_t len, shared; };
+  std::map<int, Parked> parked; int next_park = 1;
   // scratch
   float* s_lgu = nullptr;   // LM gate/up raw sums [2B][2I] (weight-stream path)
   float *s_h = nullptr, *s_qkv = nullptr;
@@ -970,6 +974,8 @@ static int build_tts_heads(vv_ctx* c) {
 
 static int upload_segs(vv_ctx* c, Codec* k, const std::vector<StateSeg>& segs) {
   k->n_segs = (int)segs.size();
+  k->state_floats = 0;
+  for (const auto& s : segs) k->state_floats += s.n;
   RET(dmalloc(c, &k->segs_dev, segs.size()));
   CK(cudaMemcpy(k->segs_dev, segs.data(), segs.size() * sizeof(StateSeg), cudaMemcpyHostToDevice));
   return 0;
@@ -1307,6 +1313,7 @@ extern "C" int vv_kv_init(vv_ctx* c, int64_t n_pages) {
     std::fill(c->shared_len.begin(), c->shared_len.end(), 0);
     for (auto& pg : c->seq_pages) pg.clear();
     c->prefixes.clear();                  // handles are never reused (next_prefix keeps counting), so old ones stay invalid
+    c->parked.clear();                    // likewise (next_park)
   }
   const auto& d = c->d;
   const size_t per_layer = (size_t)n_pages * d.num_kv_heads * KV_PAGE * d.head_dim;
@@ -1532,6 +1539,55 @@ extern "C" int64_t vv_kv_prefix_tokens(vv_ctx* c, int handle) {
 extern "C" int64_t vv_kv_seq_pages(vv_ctx* c, int seq) {
   if (!c || !c->kpool || seq < 0 || seq >= 2 * c->d.max_batch) return -1;
   return (int64_t)c->seq_pages[seq].size();
+}
+
+// ---- parked sequences: the page list moves out of the sequence with its references, and back into an empty one (any index).  Parking
+// launches nothing: an empty sequence is never read, and its stale device length is rewritten by the next length push.
+extern "C" int vv_kv_park(vv_ctx* c, int seq, int* handle) {
+  if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  if (seq < 0 || seq >= 2 * c->d.max_batch || !handle) return fail(VV_ERR_INVALID, "vv_kv_park: bad seq %d / null handle", seq);
+  if (c->kv_len_host[seq] == 0) return fail(VV_ERR_INVALID, "vv_kv_park: seq %d is empty", seq);
+  vv_ctx::Parked p;
+  p.pages = std::move(c->seq_pages[seq]);
+  p.len = c->kv_len_host[seq];
+  p.shared = c->shared_len[seq];
+  c->seq_pages[seq].clear();
+  c->kv_len_host[seq] = 0;
+  c->shared_len[seq] = 0;
+  *handle = c->next_park++;
+  c->parked.emplace(*handle, std::move(p));
+  return 0;
+}
+
+extern "C" int vv_kv_unpark(vv_ctx* c, int handle, int seq, void* stream) {
+  if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  auto it = c->parked.find(handle);
+  if (it == c->parked.end()) return fail(VV_ERR_INVALID, "vv_kv_unpark: no parked sequence %d (resumed, released, or dropped by vv_kv_init)", handle);
+  if (seq < 0 || seq >= 2 * c->d.max_batch) return fail(VV_ERR_INVALID, "bad seq %d", seq);
+  if (c->kv_len_host[seq] != 0) return fail(VV_ERR_INVALID, "vv_kv_unpark: seq %d holds %lld entries", seq, (long long)c->kv_len_host[seq]);
+  release_pages(c, seq, 0);               // the page a decode step keeps for the next entry
+  c->seq_pages[seq] = std::move(it->second.pages);
+  c->kv_len_host[seq] = it->second.len;
+  c->shared_len[seq] = it->second.shared;
+  c->parked.erase(it);
+  RET(write_page_entries(c, seq, 0, false, (cudaStream_t)stream));
+  return push_lens(c, (cudaStream_t)stream);
+}
+
+extern "C" int vv_kv_park_release(vv_ctx* c, int handle) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  auto it = c->parked.find(handle);
+  if (it == c->parked.end()) return fail(VV_ERR_INVALID, "vv_kv_park_release: no parked sequence %d", handle);
+  for (int pg : it->second.pages) unref_page(c, pg);
+  c->parked.erase(it);
+  return 0;
+}
+
+// a query: an unknown handle returns -1 without touching the last-error message
+extern "C" int64_t vv_kv_parked_pages(vv_ctx* c, int handle) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  auto it = c->parked.find(handle);
+  return it == c->parked.end() ? -1 : (int64_t)it->second.pages.size();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2991,6 +3047,41 @@ extern "C" int vv_codec_state_zero(vv_ctx* c, const int32_t* rows_host, int n, v
   CKL();
   c->launches += 2;
   return 0;
+}
+// one row's history <-> a contiguous buffer: block x < n_dec takes decoder segment x, the others encoder segment x - n_dec; a segment's
+// place in the buffer is the sum of the n of the segments before it (decoder first), read from the same tables.  save != 0: row -> buf.
+constexpr int STATE_COPY_SLICES = 4;     // CTAs per segment: the widest histories (6 x 2048 floats) would be one CTA's latency chain
+__global__ void state_copy_kernel(const StateSeg* __restrict__ dec, int n_dec, const StateSeg* __restrict__ enc, int row, float* buf,
+                                  int save) {
+  const bool in_dec = (int)blockIdx.x < n_dec;
+  const int i = in_dec ? (int)blockIdx.x : (int)blockIdx.x - n_dec;
+  size_t off = 0;
+  for (int j = 0; j < (in_dec ? i : n_dec); ++j) off += dec[j].n;
+  if (!in_dec) for (int j = 0; j < i; ++j) off += enc[j].n;
+  const StateSeg s = in_dec ? dec[i] : enc[i];
+  float* h = s.hist + (size_t)row * s.n;
+  float* b = buf + off;
+  for (int k = blockIdx.y * blockDim.x + threadIdx.x; k < s.n; k += gridDim.y * blockDim.x) {
+    if (save) b[k] = h[k];
+    else h[k] = b[k];
+  }
+}
+extern "C" int64_t vv_codec_state_floats(vv_ctx* c) {
+  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  return c->dec.state_floats + c->enc.state_floats;
+}
+static int codec_state_copy(vv_ctx* c, int row, float* buf, int save, void* stream) {
+  if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");
+  if (row < 0 || row >= c->d.max_batch || !buf) return fail(VV_ERR_INVALID, "%s: bad row %d / null buffer", save ? "vv_codec_state_save" : "vv_codec_state_load", row);
+  state_copy_kernel<<<dim3(c->dec.n_segs + c->enc.n_segs, STATE_COPY_SLICES), 256, 0, (cudaStream_t)stream>>>(c->dec.segs_dev, c->dec.n_segs,
+                                                                                                             c->enc.segs_dev, row, buf, save);
+  CKL();
+  c->launches++;
+  return 0;
+}
+extern "C" int vv_codec_state_save(vv_ctx* c, int row, float* out, void* stream) { return codec_state_copy(c, row, out, 1, stream); }
+extern "C" int vv_codec_state_load(vv_ctx* c, int row, const float* in, void* stream) {
+  return codec_state_copy(c, row, const_cast<float*>(in), 0, stream);
 }
 extern "C" int vv_codec_state_reset(vv_ctx* c, void* stream) {
   if (!c || !c->finalized) return fail(VV_ERR_STATE, "not finalized");

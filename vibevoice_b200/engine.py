@@ -394,6 +394,24 @@ class Engine:
         """pages sequence `seq` holds, shared ones included (`vv_kv_seq_pages`)."""
         return int(self.lib.vv_kv_seq_pages(self.h, int(seq)))
 
+    # parked sequences (include/vibevoice_b200.h: vv_kv_park*)
+    def kv_park(self, seq: int) -> int:
+        """move every page of non-empty sequence `seq` into a parked record (no copy); `seq` is left empty.  Returns the handle."""
+        h = C.c_int(0)
+        N.check(self.lib.vv_kv_park(self.h, int(seq), C.byref(h)), "vv_kv_park")
+        return h.value
+
+    def kv_unpark(self, handle: int, seq: int):
+        """give a parked record's pages and lengths to empty sequence `seq` (any index); the handle is used up."""
+        N.check(self.lib.vv_kv_unpark(self.h, int(handle), int(seq), self.s), "vv_kv_unpark")
+
+    def kv_park_release(self, handle: int):
+        N.check(self.lib.vv_kv_park_release(self.h, int(handle)), "vv_kv_park_release")
+
+    def kv_parked_pages(self, handle: int) -> int:
+        """pages of a live parked record, -1 when the handle is not (resumed, released, or dropped by kv_init)."""
+        return int(self.lib.vv_kv_parked_pages(self.h, int(handle)))
+
     def kv_len(self, seq: int) -> int:
         return int(self.lib.vv_kv_len(self.h, seq))
 
@@ -586,6 +604,22 @@ class Engine:
 
     def codec_state_reset(self):
         N.check(self.lib.vv_codec_state_reset(self.h, self.s))
+
+    def codec_state_save(self, row: int) -> torch.Tensor:
+        """row `row`'s committed streaming codec state (decoder and semantic encoder) as a flat fp32 device tensor, valid on the engine
+        stream (`vv_codec_state_save`)."""
+        n = N.check(int(self.lib.vv_codec_state_floats(self.h)), "vv_codec_state_floats")
+        with torch.cuda.stream(self.stream):
+            out = torch.empty(n, dtype=torch.float32, device=self.device)
+            N.check(self.lib.vv_codec_state_save(self.h, int(row), C.c_void_p(out.data_ptr()), self.s), "vv_codec_state_save")
+        return out
+
+    def codec_state_load(self, row: int, state: torch.Tensor):
+        """make `state` (from `codec_state_save`, any row) row `row`'s streaming codec state (`vv_codec_state_load`)."""
+        n = N.check(int(self.lib.vv_codec_state_floats(self.h)), "vv_codec_state_floats")
+        if state.device != self.device or state.dtype != torch.float32 or state.numel() != n or not state.is_contiguous():
+            raise ValueError("state must be %d contiguous fp32 values on %s" % (n, self.device))
+        N.check(self.lib.vv_codec_state_load(self.h, int(row), C.c_void_p(state.data_ptr()), self.s), "vv_codec_state_load")
 
     def codec_taps(self, which: int, rows):
         """One decoder (which = 0: `latent` -> `audio`) or semantic-encoder (which = 1: `audio` -> `feat`) pass with every stage boundary

@@ -9,12 +9,14 @@ live rows, so in a static batch the useful share of the work is mean length / ma
         ...
 
 Each frame runs the per-row loop body of `modeling.generate` (refresh_negative=True) for every live row, each at its own step.  After the
-frame the rows that finished are freed (both sequences to length 0, codec state zeroed) and waiting requests are admitted, oldest first,
-while the KV pool can hold their worst case.  Sampler settings are per row (`Engine.set_row_sampler`): every row pays the largest step
-count of the requests in the queue per frame.
+frame the rows that finished are freed (both sequences to length 0, codec state zeroed) and waiting requests are admitted, highest
+`priority` first and oldest first within a priority, while the KV pool can hold their worst case.  A waiting request that finds no free
+row takes the row of a running request of strictly lower priority, which is parked between frames (its K/V pages, codec state and next
+input set aside, `RequestQueue` docstring) and resumes later where it stopped.  Sampler settings are per row (`Engine.set_row_sampler`):
+every row pays the largest step count of the requests in the queue per frame.
 
-Results do not depend on batch-mates: a request's output equals `torch.manual_seed(seed); model.generate(<that request alone>, ...)` with
-`set_ddpm_inference_steps(steps)` and that solver.  Each request has its own CPU generator (diffusion noise, `randn(2, 64)[:1]` per
+Results do not depend on batch-mates or on being parked: a request's output equals `torch.manual_seed(seed); model.generate(<that
+request alone>, ...)` with `set_ddpm_inference_steps(steps)` and that solver.  Each request has its own CPU generator (diffusion noise, `randn(2, 64)[:1]` per
 diffusion frame) and device generator (voice-prompt noise, then SDE step noise), drawn in the solo run's order.
 
 `StreamingRequestQueue` does the same for the streaming-0.5B variant (`streaming.py`), with per-request audio streamers and text that
@@ -22,6 +24,7 @@ arrives while the request speaks (`push_text`).
 """
 from __future__ import annotations
 
+import bisect
 import collections
 from dataclasses import dataclass, field
 from typing import Any, Deque, Iterator, List, Optional, Tuple
@@ -49,6 +52,12 @@ class _Request:
     max_step_per_sample: int
     pages: int                          # worst-case KV pages of both sequences (with a preset: those outside its shared pages)
     preset: Any = None                  # VoicePreset or None
+    priority: int = 0
+    parked: Optional["_Row"] = None     # the row state of a request parked mid-generation (its pages stay charged)
+
+    def key(self):
+        """waiting order: highest priority first, then submission order"""
+        return (-self.priority, self.rid)
 
 
 @dataclass
@@ -67,6 +76,8 @@ class _Row:
     finished: bool = False
     reach_max: bool = False
     audio: List[torch.Tensor] = field(default_factory=list)
+    park: Optional[Tuple[int, Optional[int], torch.Tensor, torch.Tensor]] = None   # parked: (positive, negative KV handles, codec state,
+                                                                                   # embeds rows r and B + r)
 
 
 class RequestQueue:
@@ -76,7 +87,19 @@ class RequestQueue:
     prefill path: `TorchPrefill` when the model keeps one and does not default to the native prefill, else the native prefill
     (`vv_lm_prefill`) -- the token-by-token prefill of `generate()` cannot admit a row while other rows run.  A long prompt stalls every
     other row for its whole prefill; `max_prefill_tokens_per_frame` (native prefill only, rounded down to a multiple of 64) spreads it over
-    frames, which is exact because the native prefill gives the same result for any chunking."""
+    frames, which is exact because the native prefill gives the same result for any chunking.
+
+    Priorities: `submit(..., priority=p)` (default 0) serves waiting requests highest priority first, oldest first within a priority;
+    with every priority equal the queue is first in, first out.  Between frames, when the request at the head finds no free row, a
+    running request of strictly lower priority exists, and the head's worst case fits the pool beside everything already held, one row
+    is preempted: the lowest-priority row, the most recently admitted among those, of the rows that have run at least one frame.  Its
+    sequences' pages move into parked records (`Engine.kv_park`, no copy), its codec state and next-input embeddings are saved, and the
+    request goes back to the waiting list at its own priority and submission order.  Parking frees no pages (they stay charged), so it
+    helps only when rows are short; a parked request needs only a free row to resume, on any row index, and a parked request whose pages
+    keep the head waiting resumes ahead of it.  Being parked does not change a request's result.
+
+    `cancel(rid)` (between yields of `run()`) ends a waiting, admitting, running or parked request, frees its row and pages, and returns
+    what it produced so far."""
 
     def __init__(self, model, max_total_tokens: int, max_prefill_tokens_per_frame: Optional[int] = None):
         eng = model.engine
@@ -94,22 +117,24 @@ class RequestQueue:
             self._chunk = int(max_prefill_tokens_per_frame) // 64 * 64
         eng.kv_init(int(max_total_tokens))
         self._budget = eng.kv_pages - 2 * self.B          # lm_decode keeps one page for every sequence's next entry
-        self._waiting: Deque[_Request] = collections.deque()
+        self._waiting: List[_Request] = []                 # in _Request.key order
         self._next_rid = 0
         self._rows: List[Optional[_Row]] = [None] * self.B
-        self._pages_used = 0                               # the live rows' pages (shared prefixes: preset_pages())
+        self._pages_used = 0                               # the live and parked rows' pages (shared prefixes: preset_pages())
         self._admitted = 0
         self._nmax = 0
         self._modes: Optional[List[int]] = None
+        self.parks = 0                                     # rows preempted so far
 
     # ---- requests ---------------------------------------------------------------------------------------------------------------------
     def submit(self, inputs, cfg_scale: float = 1.3, steps: int = 10, solver: str = "dpmsolver++", max_new_tokens: Optional[int] = None,
                max_length_times: float = 2, seed: int = 1234, generation_config=None, logits_processor=None, audio_streamer=None,
-               stop_check_fn=None, refresh_negative: bool = True, voice_preset=None) -> int:
+               stop_check_fn=None, refresh_negative: bool = True, voice_preset=None, priority: int = 0) -> int:
         """Queue one request; `inputs` is the processor output for ONE script (+ its voices).  Returns the request id `run()` reports.
         With `voice_preset` (`model.voice_preset`) the prompt must start with the preset's prefix: the request runs no voice encoding,
         attaches the preset's shared K/V pages (prefilling them first if they are not in the pool) and is prefilled natively from there;
-        its result equals `generate(<that request>, voice_preset=voice_preset)`."""
+        its result equals `generate(<that request>, voice_preset=voice_preset)`.  `priority`: a higher one is served first and may
+        preempt running requests of lower priority (class docstring)."""
         if audio_streamer is not None:
             raise ValueError("audio_streamer is not supported by RequestQueue")
         if stop_check_fn is not None:
@@ -166,20 +191,56 @@ class RequestQueue:
             raise ValueError("max_total_tokens: the request needs up to %d KV pages, the pool has %d for requests" % (pages + shared, self._budget))
         rid = self._next_rid
         self._next_rid += 1
-        self._waiting.append(_Request(rid, ids[0], am[0].bool(), voice, float(cfg_scale), steps, solver, int(seed), max_length,
-                                      max_steps, max_step_per_sample, pages, voice_preset))
+        self._wait(_Request(rid, ids[0], am[0].bool(), voice, float(cfg_scale), steps, solver, int(seed), max_length, max_steps,
+                            max_step_per_sample, pages, voice_preset, int(priority)))
         return rid
+
+    def _wait(self, req: _Request):
+        bisect.insort(self._waiting, req, key=_Request.key)
+
+    def cancel(self, rid: int) -> VibeVoiceGenerationOutput:
+        """End request `rid` now (between yields of `run()`), whether it waits, is being admitted, runs or is parked: frees its row and
+        KV pages and returns what it produced so far (the prompt and the audio of the frames it ran)."""
+        for r, row in enumerate(self._rows):
+            if row is not None and row.req.rid == rid:
+                return self._finish(r)
+        req = next((w for w in self._waiting if w.rid == rid), None)
+        if req is None:
+            raise KeyError("request %r is not queued or live" % (rid,))
+        self._waiting.remove(req)
+        row = req.parked
+        if row is None:
+            return VibeVoiceGenerationOutput(sequences=req.ids[None].clone(), speech_outputs=[None], reach_max_step_sample=torch.tensor([False]))
+        self._drop_parked(req)
+        with torch.cuda.stream(self.eng.stream):
+            audio = torch.cat(row.audio, dim=-1) if row.audio else None
+        self.eng.sync()
+        return VibeVoiceGenerationOutput(sequences=torch.tensor([row.seq], dtype=torch.long), speech_outputs=[audio],
+                                         reach_max_step_sample=torch.tensor([row.reach_max]))
+
+    def _drop_parked(self, req: _Request):
+        """release a parked request's pages (its KV records) and its charge"""
+        hp, hn = req.parked.park[:2]
+        for h in (hp, hn):
+            if h is not None:
+                self.eng.kv_park_release(h)
+        req.parked = None
+        self._pages_used -= req.pages
+
+    def _held_rows(self) -> List[_Row]:
+        """the rows whose pages are in the pool: live ones and parked ones"""
+        return [row for row in self._rows if row is not None] + [w.parked for w in self._waiting if w.parked is not None]
 
     def _prefixes(self) -> dict:
         """handle -> pages of every shared prefix in the pool (this queue's presets, and any other preset used on the model since)."""
         return getattr(self.eng, "prefix_pages", None) or {}
 
     def preset_pages(self, extra=None) -> int:
-        """KV pages of shared prefixes: every prefix in the pool, the released ones live rows still hold, and the presets that live rows
-        build or wait for (+ `extra`'s when it is not in the pool)."""
+        """KV pages of shared prefixes: every prefix in the pool, the released ones live or parked rows still hold, and the presets that
+        live rows build or wait for (+ `extra`'s when it is not in the pool)."""
         held, pending = dict(self._prefixes()), {}
-        for row in self._rows:
-            p = None if row is None else row.req.preset
+        for row in self._held_rows():
+            p = row.req.preset
             if p is None or not p.shared:
                 continue
             if row.prefix is not None:
@@ -194,14 +255,16 @@ class RequestQueue:
         return self._pages_used + self.preset_pages(req.preset) + req.pages <= self._budget
 
     def _evict(self, req) -> bool:
-        """Release shared prefixes until the request at the head fits: first those no live or waiting request uses, then, with no row
-        live, every one but its own (their requests build them again).  Without the second step a pool filled by resident presets would
-        keep the head waiting for ever; `submit` made sure it fits beside its own preset alone.  Returns whether it fits now."""
+        """Release shared prefixes until the request at the head fits: first those no live, parked or waiting request uses, then, with
+        no row live, every one but its own and those of parked rows (their requests build them again).  Without the second step a pool
+        filled by resident presets would keep the head waiting for ever; `submit` made sure it fits beside its own preset alone.  Returns
+        whether it fits now."""
         live = any(row is not None for row in self._rows)
-        keep = {row.prefix for row in self._rows if row is not None}
+        keep = {row.prefix for row in self._held_rows()}
+        parked = {w.parked.prefix for w in self._waiting if w.parked is not None}
         own = {req.preset._handle} if req.preset is not None and req.preset.resident() else set()
         used = {w.preset._handle for w in self._waiting if w.preset is not None and w.preset.resident()}
-        for spare in ([keep | used | own] if live else [keep | used | own, own]):
+        for spare in ([keep | used | own] if live else [keep | used | own, own | parked]):
             for h in [h for h in self._prefixes() if h not in spare]:
                 self.eng.kv_prefix_release(h)
             if self._fits(req):
@@ -231,6 +294,9 @@ class RequestQueue:
         finally:
             for s in range(2 * self.B):
                 eng.kv_set_len(s, 0)
+            for w in [w for w in self._waiting if w.parked is not None]:      # dropped with the live rows when run() is left early
+                self._drop_parked(w)
+                self._waiting.remove(w)
             self._rows = [None] * self.B
             self._pages_used = 0
             eng.set_row_mode([1] * (2 * self.B))
@@ -250,14 +316,27 @@ class RequestQueue:
         while self._waiting:
             req = self._waiting[0]
             if req.max_steps <= 0:                      # generate() runs no step: the prompt comes back as it is
-                self._waiting.popleft()
+                self._waiting.pop(0)
                 done.append((req.rid, VibeVoiceGenerationOutput(sequences=req.ids[None].clone(), speech_outputs=[None],
                                                                 reach_max_step_sample=torch.tensor([False]))))
                 continue
             free = [r for r in range(self.B) if self._rows[r] is None]
-            if not free or not (self._fits(req) or self._evict(req)):
+            victim = None if free else self._victim(req)
+            if not free and victim is None:
                 break
-            self._waiting.popleft()
+            if req.parked is None and not (self._fits(req) or self._evict(req)):
+                # parked requests hold their pages whatever runs: resuming them on rows the head cannot use is how those pages come back
+                for w in [w for w in self._waiting if w.parked is not None][:len(free)]:
+                    self._waiting.remove(w)
+                    self._resume(w, free.pop(0))
+                break
+            if victim is not None:
+                self._park(victim)
+                free = [victim]
+            self._waiting.pop(0)
+            if req.parked is not None:
+                self._resume(req, free[0])
+                continue
             self._pages_used += req.pages
             r = free[0]
             if req.steps > self._nmax:
@@ -282,6 +361,45 @@ class RequestQueue:
             row.embeds = e
             self._rows[r] = row
         return done
+
+    def _victim(self, req: _Request) -> Optional[int]:
+        """The row `req` may preempt: among the rows of strictly lower priority that have run a frame, the lowest priority, then the most
+        recently admitted; None when there is none."""
+        rows = [r for r, row in enumerate(self._rows) if row is not None and row.step >= 1 and row.req.priority < req.priority]
+        return min(rows, key=lambda r: (self._rows[r].req.priority, -self._rows[r].order), default=None)
+
+    def _park(self, r: int):
+        """Set row r's request aside between frames: both sequences' pages (still charged), its codec state and its next input rows go
+        with the `_Row`, which keeps its generators, tokens, step and audio; the request waits again at its own priority and order."""
+        eng, B, row = self.eng, self.B, self._rows[r]
+        hp = eng.kv_park(r)
+        hn = eng.kv_park(B + r) if eng.kv_len(B + r) > 0 else None     # the negative sequence is empty after a <speech_start>
+        codec = eng.codec_state_save(r)
+        with torch.cuda.stream(eng.stream):
+            emb = eng.embeds[[r, B + r]]
+        eng.codec_state_zero([r])
+        row.park = (hp, hn, codec, emb)
+        row.req.parked = row
+        self._rows[r] = None
+        self.parks += 1
+        self._wait(row.req)
+
+    def _resume(self, req: _Request, r: int):
+        """Continue a parked request on free row r (any index): its pages, codec state, next input and sampler settings."""
+        eng, B, row = self.eng, self.B, req.parked
+        hp, hn, codec, emb = row.park
+        eng.set_row_sampler(r, req.steps, req.solver, req.cfg_scale)
+        eng.kv_unpark(hp, r)
+        if hn is not None:
+            eng.kv_unpark(hn, B + r)
+        eng.codec_state_load(r, codec)
+        with torch.cuda.stream(eng.stream):
+            eng.embeds[r].copy_(emb[0])
+            eng.embeds[B + r].copy_(emb[1])
+        row.park, req.parked = None, None
+        row.order = self._admitted
+        self._admitted += 1
+        self._rows[r] = row
 
     def _prefill_progress(self):
         """Prefill the admitting rows, oldest first: whole prompts, or at most max_prefill_tokens_per_frame tokens in all."""
