@@ -129,9 +129,32 @@ int64_t vv_kv_seq_pages(vv_ctx* ctx, int seq);                                 /
  * are never reused.  Every refusal returns VV_ERR_INVALID / VV_ERR_STATE and launches nothing. */
 int vv_kv_park(vv_ctx* ctx, int seq, int* handle);
 int vv_kv_unpark(vv_ctx* ctx, int handle, int seq, void* stream);
-int vv_kv_park_release(vv_ctx* ctx, int handle);                               /* drop a parked record's references */
-int64_t vv_kv_parked_pages(vv_ctx* ctx, int handle);                           /* pages of a live record, else -1 (a query: no error
-                                                                                  message is recorded) */
+int vv_kv_park_release(vv_ctx* ctx, int handle);                               /* drop a parked record's references (resident or
+                                                                                  swapped: a swapped one holds only its shared pages) */
+int64_t vv_kv_parked_pages(vv_ctx* ctx, int handle);                           /* pages of a live record in the pool, else -1 (a
+                                                                                  query: no error message is recorded) */
+
+/* ---- swapped parked records: a parked record's private pages moved to page-locked host memory, so the pool gets them back -------- *
+ * A record's private pages are its pages at index >= shared / 64: only the record holds them.  Its shared pages (a prefix's) stay in
+ * the pool with their references, so prefix pages are never moved.  vv_kv_swap_out copies K and V of every private page, every layer,
+ * into `host`, then drops the record's references to them (they return to the free list) and marks the record swapped: vv_kv_parked_pages
+ * then counts only its shared pages, and vv_kv_unpark refuses it (VV_ERR_STATE).  vv_kv_swap_in takes that many pages from the free list,
+ * copies the data back into them and makes the record resident again, its page list in the original order with the new page ids at the
+ * private positions: vv_kv_unpark then continues the sequence bit for bit.  Whole pages are copied (the slots past the length too), so
+ * no page needs zeroing.  Host layout: private page i, layer l: the K block, then the V block, of page_elems = num_kv_heads * 64 *
+ * head_dim bf16 each, at element offset ((i * num_layers + l) * 2 + kv) * page_elems; vv_kv_swap_bytes is private pages * num_layers * 2
+ * * page_elems * 2 bytes, whether the record is resident or swapped (-1 for a dead handle: a query, no error message is recorded).
+ * The copy is one kv_swap_kernel launch per 32 private pages on `stream`, through the mapped device address of `host`, which must be
+ * page-locked (cudaHostAlloc, cudaHostRegister: cudaPointerGetAttributes reports cudaMemoryTypeHost), 16-byte aligned and at least
+ * vv_kv_swap_bytes long.  The host data is complete, and `host` may be reused after swap-in, once `stream` has passed the copy.
+ * Condition: swap-out frees the pages when the copy is enqueued, not when it has run.  That is safe only while every later writer of a
+ * pool page (vv_kv_reserve's zeroing, decode appends, prefill, swap-in) is enqueued on the same stream, as for every page release.
+ * Refusals launch nothing and change nothing: a dead handle, swap-out of a swapped record or swap-in of a resident one (VV_ERR_STATE),
+ * a null, pageable or misaligned host pointer, host_bytes below vv_kv_swap_bytes (VV_ERR_INVALID), and swap-in with fewer free pages than
+ * the record needs (VV_ERR_NOMEM).  vv_kv_park_release accepts a swapped record; vv_kv_init drops swapped records with the others. */
+int64_t vv_kv_swap_bytes(vv_ctx* ctx, int handle);
+int vv_kv_swap_out(vv_ctx* ctx, int handle, void* host, int64_t host_bytes, void* stream);
+int vv_kv_swap_in(vv_ctx* ctx, int handle, const void* host, int64_t host_bytes, void* stream);
 
 /* ---- a-3: LLM decode step for pos+neg rows in ONE weight pass ---------------------------------- *
  * replaces self(**model_inputs) at :480-482 and the negative forward at :583-585.

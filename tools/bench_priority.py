@@ -7,12 +7,18 @@ Workload per model (synthetic weights, native prompt prefill, --batch rows): a b
 tools/bench_queue.py does), so both passes make the same audio.  In the "fifo" pass every request has priority 0 (today's
 first-in-first-out queue); in the "priority" pass the interactive requests have priority 1 and preempt backlog rows.
 
+The pool holds the worst case of B live rows and B parked ones by default (`--pool live+parked`), so parking never waits for pages.
+`--pool live` sizes it for the B live rows alone: then a preempting request does not fit beside the rows it preempts unless their
+pages move to host memory, and `--swap-gib X` adds a "priority_swap" pass with `RequestQueue(host_swap_bytes=X GiB)`.
+
 Reported per model and pass: the interactive requests' latency from submit to result (p50 / p90, in frames and host ms; results leave
 `run()` after a device synchronisation), total audio-s/s (CUDA events around the whole run), and in the priority pass the number of parks
 and the cost of one park plus its resume in us (CUDA events on the engine stream around each call), with the GPU's name, power limit
-and clocks read in the same run.
+and clocks read in the same run.  With swapping, also the number of swap-outs and the median cost of one swap-out and one swap-in
+(`Engine.kv_swap_out` / `kv_swap_in`, CUDA events around each call, the pinned-buffer allocation included).
 
     python tools/bench_priority.py [--presets 1.5b,7b] [--batch 8] [--backlog 24] [--interactive 12] [--prompt 256]
+                                   [--pool live+parked|live] [--swap-gib X]
 """
 import argparse
 import json
@@ -64,10 +70,11 @@ def one_model(args, preset):
     at = [args.first_arrival + i * (span - args.first_arrival) // (args.interactive + 1) for i in range(args.interactive)]
     max_new = max(frames) + 2
 
-    def run_pass(prio, scale=1):
+    def run_pass(prio, scale=1, swap_bytes=0):
         fr = [max(1, f // scale) for f in frames]
         pages = (args.prompt + max_new + 2 + 63) // 64 + (max_new + 2 + 63) // 64      # a request's worst case (RequestQueue.submit)
-        q = RequestQueue(model, max_total_tokens=2 * B * pages * 64)                     # B live rows and up to B parked ones
+        held = B if args.pool == "live" else 2 * B                                       # B live rows (and up to B parked ones)
+        q = RequestQueue(model, max_total_tokens=held * pages * 64, host_swap_bytes=swap_bytes)
         sub = lambda i, p: q.submit(dict(input_ids=prompts[i]), cfg_scale=1.3, steps=args.steps, max_new_tokens=max_new,
                                     max_length_times=1e9, seed=i, priority=p)
         rid_frames = {sub(i, 0): fr[i] for i in range(args.backlog)}
@@ -101,11 +108,13 @@ def one_model(args, preset):
             return call
         eng.read_tokens, q._frame = scripted, counted
         q._park, q._resume = ev_timed(park, "park"), ev_timed(resume, "resume")
+        q._swap_out = ev_timed(q._swap_out, "swap_out")
+        eng.kv_swap_in = ev_timed(eng.kv_swap_in, "swap_in")
         lat_f, lat_ms, audio = [], [], 0.0
         try:
             ms, outs = timed(eng, lambda: [(rid, out, n_frame[0], time.perf_counter()) for rid, out in q.run()])
         finally:
-            del eng.read_tokens
+            del eng.read_tokens, eng.kv_swap_in
         for rid, out, nf, t in outs:
             audio += out.speech_outputs[0].shape[-1] / SR
             if rid in submitted:
@@ -122,10 +131,19 @@ def one_model(args, preset):
             res["park_us_median"] = round(statistics.median(parks) * 1e3, 1)
             res["resume_us_median"] = round(statistics.median(resumes) * 1e3, 1)
             res["park_plus_resume_us"] = round((statistics.median(parks) + statistics.median(resumes)) * 1e3, 1)
+        if swap_bytes:
+            res["swaps"] = q.swaps
+            for k in ("swap_out", "swap_in"):
+                c = [ms for key, ms in costs if key == k]
+                if c:
+                    res[k + "_us_median"] = round(statistics.median(c) * 1e3, 1)
         return res
 
-    run_pass(1, scale=32)                      # warm-up: programs built, graphs captured, a park and a resume taken
+    swap = int(args.swap_gib * (1 << 30))
+    run_pass(1, scale=32, swap_bytes=swap)     # warm-up: programs built, graphs captured, a park and a resume (and a swap) taken
     out = dict(fifo=run_pass(0), priority=run_pass(1))
+    if swap:
+        out["priority_swap"] = run_pass(1, swap_bytes=swap)
     eng.close()
     del model
     torch.cuda.empty_cache()
@@ -141,11 +159,16 @@ def main():
     ap.add_argument("--prompt", type=int, default=256)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--first-arrival", type=int, default=50)
+    ap.add_argument("--pool", default="live+parked", choices=["live+parked", "live"],
+                    help="KV pool sized for B live rows and B parked ones, or for the live rows alone")
+    ap.add_argument("--swap-gib", type=float, default=0.0, help="host memory for swapped KV pages; > 0 adds a priority_swap pass")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_priority.py measures the GPU: no CUDA device")
     res = dict(tool="bench_priority", batch=args.batch, backlog=args.backlog, interactive=args.interactive, prompt_tokens=args.prompt,
                steps=args.steps, gpu=gpu_info())
+    if args.pool != "live+parked" or args.swap_gib:
+        res.update(pool=args.pool, swap_gib=args.swap_gib)
     for p in args.presets.split(","):
         res[p] = one_model(args, p)
     res["gpu_after"] = gpu_info()

@@ -64,6 +64,9 @@ SYMBOLS = {
     "vv_kv_unpark": (_I, [_P, _I, _I, _P]),
     "vv_kv_park_release": (_I, [_P, _I]),
     "vv_kv_parked_pages": (_L, [_P, _I]),
+    "vv_kv_swap_bytes": (_L, [_P, _I]),
+    "vv_kv_swap_out": (_I, [_P, _I, _P, _L, _P]),
+    "vv_kv_swap_in": (_I, [_P, _I, _P, _L, _P]),
     "vv_set_rope_inv_freq": (_I, [_P, _P, _I]),
     "vv_set_row_mode": (_I, [_P, _P, _P]),
     "vv_lm_decode": (_I, [_P, _P, _P, _P, _P, _P]),

@@ -139,7 +139,9 @@ struct vv_ctx {
   struct Prefix { std::vector<int> pages; int64_t n_tokens; };
   std::vector<int> page_ref; std::vector<int64_t> shared_len; std::map<int, Prefix> prefixes; int next_prefix = 1;
   // parked sequences: a sequence's whole page list with its lengths, holding the references it took (vv_kv_park)
-  struct Parked { std::vector<int> pages; int64_t len, shared; };
+  // host_pages: -1 while resident; once swapped out (vv_kv_swap_out), the private pages held in host memory, and `pages` keeps only the
+  // shared ones (index < shared / KV_PAGE)
+  struct Parked { std::vector<int> pages; int64_t len, shared; int host_pages = -1; };
   std::map<int, Parked> parked; int next_park = 1;
   // scratch
   float* s_lgu = nullptr;   // LM gate/up raw sums [2B][2I] (weight-stream path)
@@ -1348,6 +1350,39 @@ __global__ void page_grant_kernel(int* dst, PageVals pv, int n, int zero, bf16* 
   for (size_t i = threadIdx.x; i < page_elems / 8; i += blockDim.x) { k[i] = make_uint4(0u, 0u, 0u, 0u); v[i] = make_uint4(0u, 0u, 0u, 0u); }
 }
 
+// block (i, layer) copies the K and V rows of page pv.v[i] in that layer to (out != 0) or from host image page first + i, whose K block
+// then V block of `page_elems` bf16 each sit at element ((page * num_layers + layer) * 2 + kv) * page_elems (gridDim.y = num_layers).
+// `host` is the device address of mapped page-locked memory: one launch moves up to 32 pages of every layer with 16-byte accesses over
+// PCIe, where a cudaMemcpyAsync per block would be num_layers * 2 copies per page.  Whole pages move, the slots past a sequence's length
+// included, so pages taken for a swap-in need no zeroing.  Four loads per operand are issued before their stores to keep more of the
+// link's latency covered.
+__global__ void kv_swap_kernel(PageVals pv, int first, int out, bf16* kpool, bf16* vpool, uint4* host, size_t per_layer, size_t page_elems) {
+  const size_t o = per_layer * blockIdx.y + (size_t)pv.v[blockIdx.x] * page_elems;
+  const size_t n = page_elems / 8;
+  uint4* pk = reinterpret_cast<uint4*>(kpool + o);
+  uint4* pv_ = reinterpret_cast<uint4*>(vpool + o);
+  uint4* hk = host + ((size_t)(first + blockIdx.x) * gridDim.y + blockIdx.y) * 2 * n;
+  uint4* hv = hk + n;
+  const uint4* __restrict__ sk = out ? pk : hk;
+  const uint4* __restrict__ sv = out ? pv_ : hv;
+  uint4* __restrict__ dk = out ? hk : pk;
+  uint4* __restrict__ dv = out ? hv : pv_;
+  constexpr int U = 4;
+  for (size_t i = threadIdx.x; i < n; i += U * blockDim.x) {
+    uint4 a[U], b[U];
+#pragma unroll
+    for (int j = 0; j < U; ++j) {
+      const size_t x = i + (size_t)j * blockDim.x;
+      if (x < n) { a[j] = sk[x]; b[j] = sv[x]; }
+    }
+#pragma unroll
+    for (int j = 0; j < U; ++j) {
+      const size_t x = i + (size_t)j * blockDim.x;
+      if (x < n) { dk[x] = a[j]; dv[x] = b[j]; }
+    }
+  }
+}
+
 // page-table entries [first, end) of seq from seq_pages, 32 per launch; zero: the pages are new to seq and get K = V = 0
 static int write_page_entries(vv_ctx* c, int seq, size_t first, bool zero, cudaStream_t s) {
   const auto& pg = c->seq_pages[seq];
@@ -1563,6 +1598,7 @@ extern "C" int vv_kv_unpark(vv_ctx* c, int handle, int seq, void* stream) {
   if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
   auto it = c->parked.find(handle);
   if (it == c->parked.end()) return fail(VV_ERR_INVALID, "vv_kv_unpark: no parked sequence %d (resumed, released, or dropped by vv_kv_init)", handle);
+  if (it->second.host_pages >= 0) return fail(VV_ERR_STATE, "vv_kv_unpark: parked sequence %d is swapped out (vv_kv_swap_in first)", handle);
   if (seq < 0 || seq >= 2 * c->d.max_batch) return fail(VV_ERR_INVALID, "bad seq %d", seq);
   if (c->kv_len_host[seq] != 0) return fail(VV_ERR_INVALID, "vv_kv_unpark: seq %d holds %lld entries", seq, (long long)c->kv_len_host[seq]);
   release_pages(c, seq, 0);               // the page a decode step keeps for the next entry
@@ -1588,6 +1624,78 @@ extern "C" int64_t vv_kv_parked_pages(vv_ctx* c, int handle) {
   if (!c) return fail(VV_ERR_INVALID, "null ctx");
   auto it = c->parked.find(handle);
   return it == c->parked.end() ? -1 : (int64_t)it->second.pages.size();
+}
+
+// ---- swapped parked records: a record's private pages (index >= shared / KV_PAGE) copied to page-locked host memory and given back to
+// the free list, and later copied into pages taken from it again.  The shared pages stay in the record with their references.
+static int64_t kv_page_bytes(const vv_ctx* c) {
+  return (int64_t)c->d.num_layers * 2 * c->d.num_kv_heads * KV_PAGE * c->d.head_dim * (int64_t)sizeof(bf16);
+}
+static int private_pages(const vv_ctx::Parked& p) {
+  return p.host_pages >= 0 ? p.host_pages : (int)p.pages.size() - (int)(p.shared / KV_PAGE);
+}
+
+// a query: an unknown handle returns -1 without touching the last-error message
+extern "C" int64_t vv_kv_swap_bytes(vv_ctx* c, int handle) {
+  if (!c) return fail(VV_ERR_INVALID, "null ctx");
+  auto it = c->parked.find(handle);
+  return it == c->parked.end() ? -1 : private_pages(it->second) * kv_page_bytes(c);
+}
+
+static int kv_swap(vv_ctx* c, int handle, void* host, int64_t host_bytes, bool out, cudaStream_t s) {
+  const char* who = out ? "vv_kv_swap_out" : "vv_kv_swap_in";
+  if (!c || !c->kpool) return fail(VV_ERR_STATE, "KV pool not initialised");
+  auto it = c->parked.find(handle);
+  if (it == c->parked.end()) return fail(VV_ERR_INVALID, "%s: no parked sequence %d (resumed, released, or dropped by vv_kv_init)", who, handle);
+  vv_ctx::Parked& p = it->second;
+  if (out == (p.host_pages >= 0)) return fail(VV_ERR_STATE, "%s: parked sequence %d is %s", who, handle, out ? "already swapped out" : "resident");
+  if (!host) return fail(VV_ERR_INVALID, "%s: null host buffer", who);
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, host) != cudaSuccess || attr.type != cudaMemoryTypeHost) {
+    cudaGetLastError();                   // a pointer the runtime does not know is not an error of the context
+    return fail(VV_ERR_INVALID, "%s: the host buffer is not page-locked memory (cudaHostAlloc / cudaHostRegister / pin_memory)", who);
+  }
+  if ((uintptr_t)host % 16) return fail(VV_ERR_INVALID, "%s: the host buffer is not 16-byte aligned", who);
+  const int n = private_pages(p);
+  const int64_t need = n * kv_page_bytes(c);
+  if (host_bytes < need) return fail(VV_ERR_INVALID, "%s: host buffer of %lld bytes, the record needs %lld", who, (long long)host_bytes, (long long)need);
+  if (!out && n > (int)c->free_pages.size())
+    return fail(VV_ERR_NOMEM, "vv_kv_swap_in: parked sequence %d needs %d pages, %d are free", handle, n, (int)c->free_pages.size());
+  void* dev = nullptr;
+  if (n > 0) CK(cudaHostGetDevicePointer(&dev, host, 0));
+  const size_t first = (size_t)(p.shared / KV_PAGE);
+  if (!out) {
+    for (int i = 0; i < n; ++i) {
+      p.pages.push_back(c->free_pages.back());
+      c->free_pages.pop_back();
+      c->page_ref[p.pages.back()] = 1;
+    }
+  }
+  const auto& d = c->d;
+  const size_t page_elems = (size_t)d.num_kv_heads * KV_PAGE * d.head_dim;
+  for (int i0 = 0; i0 < n; i0 += 32) {
+    PageVals pv;
+    const int m = std::min(32, n - i0);
+    for (int i = 0; i < 32; ++i) pv.v[i] = i < m ? p.pages[first + i0 + i] : 0;
+    kv_swap_kernel<<<dim3(m, d.num_layers), 256, 0, s>>>(pv, i0, out ? 1 : 0, c->kpool, c->vpool, reinterpret_cast<uint4*>(dev),
+                                                         (size_t)c->n_pages * page_elems, page_elems);
+    CKL();
+    c->launches++;
+  }
+  if (out) {
+    for (size_t i = first; i < p.pages.size(); ++i) unref_page(c, p.pages[i]);   // free at enqueue time: see vibevoice_b200.h
+    p.pages.resize(first);
+    p.host_pages = n;
+  } else {
+    p.host_pages = -1;
+  }
+  return 0;
+}
+extern "C" int vv_kv_swap_out(vv_ctx* c, int handle, void* host, int64_t host_bytes, void* stream) {
+  return kv_swap(c, handle, host, host_bytes, true, (cudaStream_t)stream);
+}
+extern "C" int vv_kv_swap_in(vv_ctx* c, int handle, const void* host, int64_t host_bytes, void* stream) {
+  return kv_swap(c, handle, const_cast<void*>(host), host_bytes, false, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

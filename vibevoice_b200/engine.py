@@ -5,7 +5,7 @@ captured CUDA graphs are bound to, and the stream they run on.  Pure plumbing --
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Iterable, Optional, Tuple
+from typing import Dict, Iterable, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -74,6 +74,7 @@ class Engine:
         self.kv_pages = 0
         self.kv_epoch = 0                         # kv_init count: a prefix made in an earlier pool is gone
         self.prefix_pages: Dict[int, int] = {}
+        self._host_keep: List[torch.Tensor] = []  # pinned buffers a swap kernel may still access: dropped at the next sync()
         self.stream = torch.cuda.Stream(device=self.device)
         H, B = config.decoder_config.hidden_size, max_batch
         dev = self.device
@@ -412,6 +413,35 @@ class Engine:
         """pages of a live parked record, -1 when the handle is not (resumed, released, or dropped by kv_init)."""
         return int(self.lib.vv_kv_parked_pages(self.h, int(handle)))
 
+    # swapped parked records (include/vibevoice_b200.h: vv_kv_swap*)
+    @property
+    def kv_page_bytes(self) -> int:
+        """host bytes of one page: K and V of every layer"""
+        dc = self.config.decoder_config
+        return dc.num_hidden_layers * 2 * dc.num_key_value_heads * 64 * dc.head_dim * 2
+
+    def kv_swap_bytes(self, handle: int) -> int:
+        """host bytes of a parked record's private pages, resident or swapped; -1 when the handle is not live."""
+        return int(self.lib.vv_kv_swap_bytes(self.h, int(handle)))
+
+    def kv_swap_out(self, handle: int) -> torch.Tensor:
+        """copy parked record `handle`'s private pages into a new pinned uint8 tensor and give the pages back to the pool; the tensor
+        holds them once the engine stream has passed the copy."""
+        n = self.kv_swap_bytes(handle)
+        if n < 0:
+            raise N.VVError("kv_swap_out: no parked sequence %d" % handle)
+        buf = torch.empty(n, dtype=torch.uint8, pin_memory=True)
+        N.check(self.lib.vv_kv_swap_out(self.h, int(handle), C.c_void_p(buf.data_ptr()), n, self.s), "vv_kv_swap_out")
+        self._host_keep.append(buf)
+        return buf
+
+    def kv_swap_in(self, handle: int, buf: torch.Tensor):
+        """copy `buf` (from `kv_swap_out(handle)`) into pages taken from the pool; the record is resident again (`kv_unpark` works)."""
+        if buf.dtype != torch.uint8 or buf.device.type != "cpu" or not buf.is_contiguous():
+            raise ValueError("buf must be the contiguous pinned uint8 tensor kv_swap_out returned")
+        N.check(self.lib.vv_kv_swap_in(self.h, int(handle), C.c_void_p(buf.data_ptr()), buf.numel(), self.s), "vv_kv_swap_in")
+        self._host_keep.append(buf)      # the pinned caching allocator must not hand the block out while the copy reads it
+
     def kv_len(self, seq: int) -> int:
         return int(self.lib.vv_kv_len(self.h, seq))
 
@@ -671,3 +701,4 @@ class Engine:
 
     def sync(self):
         self.stream.synchronize()
+        self._host_keep = []

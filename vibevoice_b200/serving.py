@@ -78,6 +78,8 @@ class _Row:
     audio: List[torch.Tensor] = field(default_factory=list)
     park: Optional[Tuple[int, Optional[int], torch.Tensor, torch.Tensor]] = None   # parked: (positive, negative KV handles, codec state,
                                                                                    # embeds rows r and B + r)
+    host: Optional[List[Any]] = None    # swapped out: the pinned host copies of the parked records' private pages (positive, negative)
+    host_bytes: int = 0                 # their size, charged against host_swap_bytes
 
 
 class RequestQueue:
@@ -94,14 +96,24 @@ class RequestQueue:
     running request of strictly lower priority exists, and the head's worst case fits the pool beside everything already held, one row
     is preempted: the lowest-priority row, the most recently admitted among those, of the rows that have run at least one frame.  Its
     sequences' pages move into parked records (`Engine.kv_park`, no copy), its codec state and next-input embeddings are saved, and the
-    request goes back to the waiting list at its own priority and submission order.  Parking frees no pages (they stay charged), so it
-    helps only when rows are short; a parked request needs only a free row to resume, on any row index, and a parked request whose pages
-    keep the head waiting resumes ahead of it.  Being parked does not change a request's result.
+    request goes back to the waiting list at its own priority and submission order.  Parking alone frees no pages (they stay charged): a
+    parked request needs only a free row to resume, on any row index, and a parked request whose pages keep the head waiting resumes
+    ahead of it.  Being parked does not change a request's result.
+
+    Swapping (`host_swap_bytes` > 0) makes preemption free pool pages too, so a pool sized for the live rows is enough.  When the head
+    does not fit the pool between frames (a new request, or a swapped one that needs its pages back), the queue moves the private KV
+    pages of lower-priority requests to pinned host memory (`Engine.kv_swap_out`) and uncharges their worst case.  Candidates, in order:
+    the row the head preempts, if it has no free row; parked requests of strictly lower priority; then running rows of strictly lower
+    priority that have run a frame (parked first); lowest priority first and most recently admitted first within a priority.  A candidate
+    whose pages would overflow the host budget is skipped.  The queue swaps the shortest run of candidates after which the head fits, and
+    nothing when none does.  A swapped request is charged its actual bytes against `host_swap_bytes`; it resumes once it is the head, a
+    row is free and its worst case fits the pool again (`Engine.kv_swap_in`).  Shared preset pages, codec state and next-input embeddings
+    stay on the device.  With `host_swap_bytes` = 0 nothing is swapped.
 
     `cancel(rid)` (between yields of `run()`) ends a waiting, admitting, running or parked request, frees its row and pages, and returns
     what it produced so far."""
 
-    def __init__(self, model, max_total_tokens: int, max_prefill_tokens_per_frame: Optional[int] = None):
+    def __init__(self, model, max_total_tokens: int, max_prefill_tokens_per_frame: Optional[int] = None, host_swap_bytes: int = 0):
         eng = model.engine
         if eng is None or not eng.finalized:
             raise N.VVError("weights not loaded")
@@ -125,6 +137,11 @@ class RequestQueue:
         self._nmax = 0
         self._modes: Optional[List[int]] = None
         self.parks = 0                                     # rows preempted so far
+        if int(host_swap_bytes) < 0:
+            raise ValueError("host_swap_bytes must be >= 0 (got %r)" % (host_swap_bytes,))
+        self._host_budget = int(host_swap_bytes)
+        self.swaps = 0                                     # parked requests swapped out so far
+        self.host_bytes_used = 0                           # host bytes of the swapped requests' pages
 
     # ---- requests ---------------------------------------------------------------------------------------------------------------------
     def submit(self, inputs, cfg_scale: float = 1.3, steps: int = 10, solver: str = "dpmsolver++", max_new_tokens: Optional[int] = None,
@@ -219,13 +236,22 @@ class RequestQueue:
                                          reach_max_step_sample=torch.tensor([row.reach_max]))
 
     def _drop_parked(self, req: _Request):
-        """release a parked request's pages (its KV records) and its charge"""
-        hp, hn = req.parked.park[:2]
+        """release a parked request's pages (its KV records), its host copies and its charge"""
+        row = req.parked
+        hp, hn = row.park[:2]
         for h in (hp, hn):
             if h is not None:
                 self.eng.kv_park_release(h)
         req.parked = None
-        self._pages_used -= req.pages
+        if row.host is not None:
+            self.host_bytes_used -= row.host_bytes
+            row.host, row.host_bytes = None, 0
+        else:
+            self._pages_used -= req.pages
+
+    @staticmethod
+    def _swapped(req: _Request) -> bool:
+        return req.parked is not None and req.parked.host is not None
 
     def _held_rows(self) -> List[_Row]:
         """the rows whose pages are in the pool: live ones and parked ones"""
@@ -251,8 +277,10 @@ class RequestQueue:
             pending[id(extra)] = extra.pages
         return sum(held.values()) + sum(pending.values())
 
-    def _fits(self, req) -> bool:
-        return self._pages_used + self.preset_pages(req.preset) + req.pages <= self._budget
+    def _fits(self, req, freed: int = 0) -> bool:
+        """whether `req`'s worst case fits beside everything held, less `freed` pages (a parked request holds its shared pages)"""
+        extra = req.preset if req.parked is None else None
+        return self._pages_used - freed + self.preset_pages(extra) + req.pages <= self._budget
 
     def _evict(self, req) -> bool:
         """Release shared prefixes until the request at the head fits: first those no live, parked or waiting request uses, then, with
@@ -299,6 +327,7 @@ class RequestQueue:
                 self._waiting.remove(w)
             self._rows = [None] * self.B
             self._pages_used = 0
+            self.host_bytes_used = 0
             eng.set_row_mode([1] * (2 * self.B))
             eng.sampler_per_row(0)
             eng.sync()
@@ -324,13 +353,14 @@ class RequestQueue:
             victim = None if free else self._victim(req)
             if not free and victim is None:
                 break
-            if req.parked is None and not (self._fits(req) or self._evict(req)):
+            if (req.parked is None or self._swapped(req)) and not (self._fits(req) or self._evict(req) or self._swap_for(req, victim)):
                 # parked requests hold their pages whatever runs: resuming them on rows the head cannot use is how those pages come back
-                for w in [w for w in self._waiting if w.parked is not None][:len(free)]:
+                for w in [w for w in self._waiting if w.parked is not None and not self._swapped(w)][:len(free)]:
                     self._waiting.remove(w)
                     self._resume(w, free.pop(0))
                 break
-            if victim is not None:
+            free = [r for r in range(self.B) if self._rows[r] is None]      # _swap_for may have parked rows, the victim among them
+            if not free:
                 self._park(victim)
                 free = [victim]
             self._waiting.pop(0)
@@ -384,10 +414,65 @@ class RequestQueue:
         self.parks += 1
         self._wait(row.req)
 
+    def _swap_for(self, req: _Request, victim: Optional[int]) -> bool:
+        """Swap out lower-priority requests until `req` fits the pool (class docstring): plan the shortest run of candidates first, then
+        park the running ones among them and swap every one.  Returns whether anything was swapped (then `req` fits)."""
+        if self._host_budget <= 0:
+            return False
+        order = lambda row: (row.req.priority, -row.order)
+        parked = sorted((w.parked for w in self._waiting if w.parked is not None and w.parked.host is None and w.priority < req.priority),
+                        key=order)
+        running = sorted((row for r, row in enumerate(self._rows)
+                          if row is not None and r != victim and row.step >= 1 and row.req.priority < req.priority), key=order)
+        room, freed, plan = self._host_budget - self.host_bytes_used, 0, []
+        for row in ([self._rows[victim]] if victim is not None else []) + parked + running:
+            n = self._private_bytes(row)
+            if n > room:
+                continue
+            plan.append(row)
+            room -= n
+            freed += row.req.pages
+            if self._fits(req, freed):
+                break
+        else:
+            return False
+        for row in plan:
+            if row.park is None:
+                self._park(next(r for r, x in enumerate(self._rows) if x is row))
+            self._swap_out(row)
+        return True
+
+    def _private_bytes(self, row: _Row) -> int:
+        """host bytes a swap-out of `row` would take now: its parked records' private pages, or those its sequences would park"""
+        eng, B = self.eng, self.B
+        if row.park is not None:
+            return sum(eng.kv_swap_bytes(h) for h in row.park[:2] if h is not None)
+        r = next(r for r, x in enumerate(self._rows) if x is row)
+        pages = eng.kv_seq_pages(r) - (row.req.preset.pages if row.prefix is not None else 0)
+        if eng.kv_len(B + r) > 0:                       # _park parks the negative sequence only when it holds entries
+            pages += eng.kv_seq_pages(B + r)
+        return pages * eng.kv_page_bytes
+
+    def _swap_out(self, row: _Row):
+        """move parked `row`'s private pages to pinned host memory: its worst case leaves the pool charge, its bytes join the host's"""
+        row.host_bytes = self._private_bytes(row)
+        row.host = [None if h is None else self.eng.kv_swap_out(h) for h in row.park[:2]]
+        self._pages_used -= row.req.pages
+        self.host_bytes_used += row.host_bytes
+        self.swaps += 1
+
     def _resume(self, req: _Request, r: int):
-        """Continue a parked request on free row r (any index): its pages, codec state, next input and sampler settings."""
+        """Continue a parked request on free row r (any index): its pages (copied back first when swapped), codec state, next input
+        and sampler settings."""
         eng, B, row = self.eng, self.B, req.parked
         hp, hn, codec, emb = row.park
+        if row.host is not None:
+            for h, buf in zip((hp, hn), row.host):
+                if h is not None:
+                    eng.kv_swap_in(h, buf)
+            self._pages_used += req.pages
+            self.host_bytes_used -= row.host_bytes
+            row.host, row.host_bytes = None, 0
         eng.set_row_sampler(r, req.steps, req.solver, req.cfg_scale)
         eng.kv_unpark(hp, r)
         if hn is not None:
